@@ -313,6 +313,17 @@ struct DevSchemaBuf {
   void free_all() { cudaFree(d_fields); cudaFree(d_names); cudaFree(d_ht); cudaFree(d_var_field); cudaFree(d_templates); cudaFree(d_tile_consts); }
 };
 
+// Raises Kernel's opt-in dynamic shared memory to `smem` bytes on the current device, once per device and size
+template <auto Kernel>
+static cudaError_t raise_dyn_smem(size_t smem) {
+  static size_t granted[64] = {0};                      // per device
+  int dev = 0; cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64 || granted[dev] >= smem) return cudaSuccess;
+  cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e == cudaSuccess) granted[dev] = smem;
+  return e;
+}
+
 #include "api_decode.inc"
 
 // ---------------------------------------------------------------------------------------------

@@ -224,225 +224,3 @@ __global__ void __launch_bounds__(ENC_TILE_THREADS, 3) encode_tile_kernel(EncTil
     if (lane < tl) d[hm + 4 * words + lane] = (uint8_t)T.u8(so + 4 * words + lane);
   }
 }
-
-// ---------------------------------------------------------------------------------------------
-// The whole encoder in ONE kernel: sizes, output offsets, entries, CRC framing, copy-out.
-//
-// encode_tile_size_kernel -> scan -> (host sync) -> encode_tile_kernel reads the columns twice, carries the Feature
-// sizes through HBM and stops the stream in the middle.  Here a tile of 32 rows computes its sizes in shared memory,
-// obtains the byte offset of its first record from the tiles before it with a decoupled look-back (every tile
-// publishes its byte count, then its inclusive prefix; a tile sums its predecessors' counts back to the nearest
-// published prefix, 32 predecessors per step) and emits.  Tiles take their index from a ticket counter, so every
-// predecessor of a running tile is itself running or finished: the look-back cannot wait on a tile that has not started.
-// The slot size is speculated from the previous call (a larger row sets the overflow flag and the host falls back to the
-// two-pass path); the output buffer is sized from a safe bound computed on the host from the column metadata.
-// ---------------------------------------------------------------------------------------------
-struct EncFusedArgs {
-  DevSchema sch;
-  const EncCol* cols;
-  uint32_t n_rows;
-  uint32_t n_tiles;
-  const CrcTables* tabs;
-  uint8_t* out;
-  unsigned long long out_cap;
-  uint32_t slot;                       // bytes per record slot, 4 (mod 128)
-  unsigned long long* tile_state;      // [n_tiles] (flag << 62) | bytes; flag 1: this tile's bytes, 2: inclusive prefix; zeroed per call
-  uint32_t* ticket;                    // [0], zeroed per call
-  uint32_t* small;                     // [0] atomicMin first null-in-non-nullable row, [1] overflow, [2..3] total bytes, [4] atomicMax framed record size
-  uint32_t names_bytes;
-};
-
-#define ENC_LB_AGG (1ull << 62)
-#define ENC_LB_PFX (2ull << 62)
-#define ENC_LB_VAL ((1ull << 62) - 1)
-
-__global__ void __launch_bounds__(ENC_TILE_THREADS, 3) encode_fused_kernel(EncFusedArgs A) {
-  extern __shared__ __align__(128) uint8_t esm[];
-  uint32_t* g5 = reinterpret_cast<uint32_t*>(esm);
-  const uint32_t* xp16 = g5 + 512;
-  uint32_t* scrc = g5 + 1024;
-  uint32_t* sgrp = scrc + 32;
-  const uint32_t nf = (uint32_t)A.sch.n_fields;
-  uint16_t* vsz = reinterpret_cast<uint16_t*>(sgrp + 32);
-  uint16_t* eoff = vsz + nf * 32;
-  uint8_t* meta = esm + 4096 + 128 + 128 + ((nf * 32 * 2 * 2 + 15u) & ~15u);
-  DevField* sfd = reinterpret_cast<DevField*>(meta);
-  EncCol* scol = reinterpret_cast<EncCol*>(meta + ((nf * (uint32_t)sizeof(DevField) + 15u) & ~15u));
-  uint8_t* snames = meta + ((nf * (uint32_t)sizeof(DevField) + 15u) & ~15u) + ((nf * (uint32_t)sizeof(EncCol) + 15u) & ~15u);
-  uint8_t* slots = meta + enc_tile_meta_bytes(nf, A.names_bytes);
-  __shared__ uint32_t s_tile, s_bad, s_total, s_row[ENC_TILE_ROWS];
-  __shared__ unsigned long long s_base;
-  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (threadIdx.x == 0) { s_tile = atomicAdd(A.ticket, 1u); s_bad = 0; }
-  __syncthreads();
-  const uint32_t tile = s_tile;
-  const uint32_t row0 = tile * ENC_TILE_ROWS;
-  const uint32_t rows = min((uint32_t)ENC_TILE_ROWS, A.n_rows - row0);
-  const bool active = lane < rows;
-  const uint32_t row = row0 + lane;
-  {
-    const uint32_t* g = A.tabs->g5;
-    for (uint32_t i = threadIdx.x; i < 1024; i += ENC_TILE_THREADS) g5[i] = g[i];
-    if (threadIdx.x < 32) { scrc[threadIdx.x] = 0; sgrp[threadIdx.x] = 0; }
-    const uint32_t* gf = reinterpret_cast<const uint32_t*>(A.sch.fields);            // fields, column pointers, names: see encode_tile_kernel
-    uint32_t* df = reinterpret_cast<uint32_t*>(sfd);
-    for (uint32_t i = threadIdx.x; i < nf * (uint32_t)(sizeof(DevField) / 4); i += ENC_TILE_THREADS) df[i] = gf[i];
-    const uint32_t* gc = reinterpret_cast<const uint32_t*>(A.cols);
-    uint32_t* dc = reinterpret_cast<uint32_t*>(scol);
-    for (uint32_t i = threadIdx.x; i < nf * (uint32_t)(sizeof(EncCol) / 4); i += ENC_TILE_THREADS) dc[i] = gc[i];
-    for (uint32_t i = threadIdx.x; i < A.names_bytes; i += ENC_TILE_THREADS) snames[i] = A.sch.names[i];
-  }
-  __syncthreads();
-  // ---- sizes: warp w takes fields w, w+W, ... of row `lane` ----
-  {
-    uint32_t sum = 0;
-    bool null_err = false, big = false;
-    for (uint32_t f = wid; f < nf; f += ENC_TILE_WARPS) {
-      const DevField& fd = sfd[f];
-      const uint32_t V = active ? cell_value_size(fd, scol[f], row) : 0xffffffffu;
-      if (V == 0xffffffffu) { if (active && !fd.nullable) null_err = true; vsz[f * 32 + lane] = (uint16_t)0xffff; }
-      else {
-        if (V >= 0xffffu) big = true;
-        vsz[f * 32 + lane] = (uint16_t)min(V, 0xfffeu);
-        sum += entry_total(fd, V);
-      }
-    }
-    if (sum) atomicAdd(&sgrp[lane], sum);
-    if (null_err) atomicMin(A.small, row);                               // NullPointerException (:29-31)
-    if (big) s_bad = 1;
-  }
-  __syncthreads();
-  const uint32_t G = sgrp[lane];
-  const uint32_t ghdr = 1 + vsize32(G);
-  const uint32_t plen = ghdr + G;
-  const uint32_t flen = active ? 16 + plen : 0;
-  if (wid == 0) {
-    if (active && flen > A.slot) s_bad = 1;                              // does not fit its slot: two-pass path
-    uint32_t acc = 0;
-    for (uint32_t f = 0; f < nf; ++f) {
-      const uint32_t V = vsz[f * 32 + lane];
-      eoff[f * 32 + lane] = (uint16_t)min(acc, 0xffffu);
-      if (V != 0xffffu) acc += entry_total(sfd[f], V);
-    }
-    uint32_t T;
-    s_row[lane] = warp_excl_scan_u32(flen, T);
-    const uint32_t mx = __reduce_max_sync(0xffffffffu, flen);
-    if (lane == 0) atomicMax(A.small + 4, mx);
-    // this tile's byte count is known now: publish it, so that later tiles never wait for more than our size phase
-    s_total = T;
-    if (lane == 0 && tile != 0) *reinterpret_cast<volatile unsigned long long*>(&A.tile_state[tile]) = ENC_LB_AGG | (unsigned long long)T;
-  }
-  // ---- decoupled look-back (warp 0): bytes of all earlier tiles -> offset of this tile's first record ----
-  auto look_back = [&]() {
-    const uint32_t T = s_total;
-    unsigned long long excl = 0;
-    if (tile == 0) {
-      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(&A.tile_state[0]) = ENC_LB_PFX | (unsigned long long)T;
-    } else {
-      int64_t j = (int64_t)tile - 1;
-      for (;;) {
-        const int64_t k = j - (int64_t)lane;
-        unsigned long long v = ENC_LB_PFX;                               // before tile 0: prefix 0
-        if (k >= 0) {
-          uint32_t spins = 0;
-          while (((v = *reinterpret_cast<volatile unsigned long long*>(&A.tile_state[k])) >> 62) == 0) {
-            if (++spins > (1u << 24)) __trap();                          // a lost predecessor must fail loudly, not hang
-            __nanosleep(20);
-          }
-        }
-        const uint32_t pm = __ballot_sync(0xffffffffu, (v >> 62) == 2);
-        const uint32_t upto = pm ? (uint32_t)__ffs((int)pm) - 1 : 31;    // nearest predecessor that holds a prefix
-        unsigned long long part = lane <= upto ? (v & ENC_LB_VAL) : 0ull;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-        excl += part;
-        if (pm) break;
-        j -= 32;
-      }
-      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(&A.tile_state[tile]) = ENC_LB_PFX | (excl + T);
-    }
-    if (lane == 0) {
-      s_base = excl;
-      if (excl + T > A.out_cap) s_bad = 1;
-      if (tile == A.n_tiles - 1) { A.small[2] = (uint32_t)(excl + T); A.small[3] = (uint32_t)((excl + T) >> 32); }
-    }
-  };
-  __syncthreads();
-  if (s_bad) {                                                          // the host re-runs the batch through the two-pass path
-    if (wid == 0) look_back();                                          // later tiles still need our prefix
-    if (threadIdx.x == 0) atomicOr(A.small + 1, 1u);
-    return;
-  }
-  uint8_t* rec = slots + lane * A.slot;
-  // ---- entries ----
-  if (active) {
-    for (uint32_t f = wid; f < nf; f += ENC_TILE_WARPS) {
-      const uint32_t V = vsz[f * 32 + lane];
-      if (V == 0xffffu) continue;                                        // null: the feature is omitted (:29)
-      const DevField& fd = sfd[f];
-      const EncCol& c = scol[f];
-      uint8_t* p = rec + 12 + ghdr + eoff[f * 32 + lane];
-      const uint32_t E = 1 + vsize32(fd.name_len) + fd.name_len + 1 + vsize32(V) + V;
-      *p++ = 0x0A; p = put_varint(p, E);
-      *p++ = 0x0A; p = put_varint(p, fd.name_len);
-      const uint8_t* nm = snames + fd.name_off;
-      for (uint32_t k = 0; k < fd.name_len; ++k) p[k] = nm[k];
-      p += fd.name_len;
-      *p++ = 0x12; p = put_varint(p, V);
-      if (fd.depth == 0) emit_feature(p, fd, c, (int32_t)row, (int32_t)row + 1);
-      else emit_feature(p, fd, c, c.off[0][row], c.off[0][row + 1]);
-    }
-    if (wid == 0) {                                                      // wrapper: setFeatures is always called (:33)
-      uint8_t* p = rec + 12;
-      *p++ = 0x0A; put_varint(p, G);
-    }
-  }
-  __syncthreads();
-  // ---- CRC-32C of the payload: every warp folds a share of the 16-byte chunks of record `lane` ----
-  Tile T;
-  T.b = slots;
-  T.s = smem_u32(slots);
-  const uint32_t pay = lane * A.slot + 12;
-  const uint32_t K = plen >> 4;
-  if (active) {
-    const uint32_t k0 = K * wid / ENC_TILE_WARPS, k1 = K * (wid + 1) / ENC_TILE_WARPS;
-    uint32_t c = wid == 0 ? 0xFFFFFFFFu : 0u;
-    for (uint32_t k = k0; k < k1; ++k) {
-      const uint32_t o = pay + 16 * k;
-      const uint32_t w0 = T.w32(o), w1 = T.w32(o + 4), w2 = T.w32(o + 8), w3 = T.w32(o + 12);
-      c = crc_fold8(g5, c, w0, w1);
-      c = crc_fold8(g5, c, w2, w3);
-    }
-    if (c) atomicXor(&scrc[lane], K - k1 ? gf2_mulmod(xp16[K - k1], c) : c);
-  }
-  __syncthreads();
-  if (wid == 0 && active) {
-    uint32_t c = scrc[lane];
-    for (uint32_t o = pay + 16 * K; o < pay + plen; ++o) c = crc_byte(g5, c, T.u8(o));
-    const uint32_t fc = crc_mask(~c);
-    const uint32_t hc = crc_mask(~crc_fold8(g5, 0xFFFFFFFFu, plen, 0u));
-    uint32_t* h = reinterpret_cast<uint32_t*>(rec);
-    h[0] = plen; h[1] = 0; h[2] = hc;
-    uint8_t* ft = rec + 12 + plen;
-    for (int i = 0; i < 4; ++i) ft[i] = (uint8_t)(fc >> (8 * i));
-  }
-  if (wid == 0) look_back();                                            // by now the earlier tiles have usually published
-  __syncthreads();
-  if (s_bad) { if (threadIdx.x == 0) atomicOr(A.small + 1, 1u); return; }
-  // ---- copy-out ----
-  uint8_t* dst0 = A.out + s_base;
-  for (uint32_t r = wid; r < rows; r += ENC_TILE_WARPS) {
-    const uint32_t s0 = r * A.slot;                                           // 4-byte aligned
-    const uint32_t flen = 16 + T.w32(s0);                                     // the framed length is in the record's own header
-    uint8_t* d = dst0 + s_row[r];
-    const uint32_t hm = min(flen, (0u - (uint32_t)reinterpret_cast<uintptr_t>(d)) & 3u);
-    if (lane < hm) d[lane] = (uint8_t)T.u8(s0 + lane);
-    const uint32_t words = (flen - hm) >> 2;
-    const uint32_t so = s0 + hm, sh = (so & 3u) * 8u, sa = so & ~3u;
-    uint32_t* dw = reinterpret_cast<uint32_t*>(d + hm);
-    if (sh == 0) for (uint32_t i = lane; i < words; i += 32) dw[i] = T.w32(sa + 4 * i);
-    else for (uint32_t i = lane; i < words; i += 32) dw[i] = __funnelshift_r(T.w32(sa + 4 * i), T.w32(sa + 4 * i + 4), sh);
-    const uint32_t tl = (flen - hm) & 3u;
-    if (lane < tl) d[hm + 4 * words + lane] = (uint8_t)T.u8(so + 4 * words + lane);
-  }
-}

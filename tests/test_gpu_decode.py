@@ -233,7 +233,7 @@ def test_fast_path_learns_then_speculates_then_recovers(native, oracle):
         dec.close()
 
 
-@pytest.mark.parametrize("env", [{"TFR_DISABLE_FAST": "1"}, {"TFR_DISABLE_SPECULATION": "1"}, {}])
+@pytest.mark.parametrize("env", [{"TFR_DISABLE_FAST": "1"}, {}])
 def test_path_variants_agree(native, oracle, env, monkeypatch):
     """general path only / other tile geometries: same bits"""
     from oracle.corpus import cfg2_columns, mixed_columns

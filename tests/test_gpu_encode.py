@@ -215,18 +215,17 @@ def test_tile_emit_shapes(native, oracle):
         assert got2 == want, _diff(got2, want)
 
 
-def test_one_kernel_encoder_after_the_first_call(native, oracle, monkeypatch):
-    """With TFR_FUSED_ENCODE=1 the second and later calls of an encoder take the one-kernel path (sizes + look-back offsets
-    + emit), with the slot size learned from the previous call: same bytes; a batch with a much larger row falls back and
-    re-learns; a null in a non-nullable column is reported at the same row."""
-    monkeypatch.setenv("TFR_FUSED_ENCODE", "1")
+def test_encoder_reused_across_row_sizes(native, oracle):
+    """One encoder, many calls: row counts that fill no, one or many tiles, other varint widths, ragged rows with nulls, a
+    batch with one row far larger than the ones before: same bytes as the oracle; a null in a non-nullable column is
+    reported at the same row, and the encoder goes on encoding."""
     from oracle.corpus import cfg2_columns, mixed_columns
     rng = np.random.default_rng(9)
     sch, cols = cfg2_columns(3000, seed=77)
     want, rc, _ = oracle.encode(cols, sch)
     enc = native.Encoder(sch, 0)
     try:
-        for _ in range(3):                                         # 1: two passes (learn), 2-3: one kernel
+        for _ in range(3):
             assert enc.encode(cols) == want
         sch2, cols2 = cfg2_columns(1, seed=78)                     # a single row: one partial tile
         want2, _, _ = oracle.encode(cols2, sch2)
@@ -236,7 +235,7 @@ def test_one_kernel_encoder_after_the_first_call(native, oracle, monkeypatch):
         assert enc.encode(cols3) == want3
     finally:
         enc.close()
-    # ragged rows, nulls, strings; then one row far larger than anything seen before (slot overflow -> fallback -> re-learn)
+    # ragged rows, nulls, strings; then one row far larger than anything seen before
     schm = StructType([StructField("a", LongType()), StructField("s", StringType()), StructField("v", ArrayType(LongType())),
                        StructField("f", ArrayType(FloatType())), StructField("b", ArrayType(BinaryType()))])
     def rows(n, big=None):
@@ -258,7 +257,7 @@ def test_one_kernel_encoder_after_the_first_call(native, oracle, monkeypatch):
             assert g == w, _diff(g, w)
     finally:
         enc.close()
-    # NullPointerException on the one-kernel path
+    # NullPointerException on an encoder that has encoded before
     schn = StructType([StructField("ok", LongType()), StructField("NonNullLabel", ArrayType(FloatType()), nullable=False)])
     good = A.columns_from_rows(schn, [(i, [1.0 * i]) for i in range(100)])
     bad = A.columns_from_rows(schn, [(i, None if i in (41, 77) else [1.0 * i]) for i in range(100)])
