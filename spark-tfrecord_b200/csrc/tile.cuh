@@ -19,12 +19,19 @@
 //      words, field table, entry templates, names), which api.cu keeps in HBM in exactly the shared-memory layout.
 //   2. role split over the same staged bytes: the C CRC warps each fold a third of the 16-byte chunks of record
 //      `lane` (aligned 128-bit loads, 13 conflict-free 5-bit table lookups per 8 bytes) and combine through one GF(2)
-//      shift each; parse warp w owns the map entries with index = w mod W of record `lane`: it fully parses those and
-//      only hops over the others (`0A elen` -> p += elen).  An owned entry is first matched against a per-field
-//      TEMPLATE of its constant bytes (0A ? 0A klen key 12 ? kind ?: masked word compares), which also fixes the
-//      Feature kind and list length; only when that fails is it parsed byte by byte (hash lookup of the key, full
-//      checks).  Shared-memory capacity limits how many records an SM can stage, so more dependent chains per staged
-//      record = more warps to hide latency, and no single warp's chain is the tile's critical path.
+//      shift each.  Parse warp w owns the map entries with index = w mod W of record `lane` and fully parses them.  In
+//      the 12 + 3 warp kernels the last parse warp first walks the map-entry chain of record `lane` once (`0A elen` ->
+//      p += elen) and writes where every entry starts into a shared-memory ENTRY TABLE (16-bit offsets from the payload,
+//      one row per entry index, lane = record: conflict-free rows); the parse warps wait for it at a named barrier and
+//      then go straight to each of their entries.  (Entries past the table's rows -- features the reader's schema
+//      prunes -- or past 64 KiB of payload are reached by hopping on from the last entry the table holds.)  In the 4 + 1
+//      warp kernel (small records: a tile's life is a latency chain that a walk in front of a barrier lengthens) each
+//      warp hops from one of its entries to the next (`0A elen` -> p += elen, W - 1 hops).  An owned entry is first
+//      matched against a per-field TEMPLATE of its constant bytes (0A ? 0A klen key 12 ? kind ?: masked word
+//      compares), which also fixes the Feature kind and list length; only when that fails is it parsed byte by byte
+//      (hash lookup of the key, full checks).  Shared-memory capacity limits how many records an SM can stage, so more
+//      dependent chains per staged record = more warps to hide latency, and no single warp's chain is the tile's
+//      critical path.
 //   3. lane = row, rows are 32-aligned: every column store of the warp covers 32 consecutive rows
 //      (coalesced by construction, no transpose) and validity bitmaps are one __ballot_sync per field.
 //   4. variable-width columns either write element counts + source offsets (scan + decode_pass2_kernel
@@ -199,6 +206,16 @@ __device__ __forceinline__ bool t_len(const Tile& t, uint32_t& p, uint32_t end, 
   }
   return false;
 }
+// map entry at p (`0A elen ...`, p < end) -> the next one: one byte load + add, the full length varint only for entries of
+// 128+ bytes.  The tag and the contents are the owner's to check; false if the length varint runs past `end`.
+__device__ __forceinline__ bool t_next_entry(const Tile& t, uint32_t& p, uint32_t end) {
+  const int32_t b1 = t.i8(p + 1);
+  if (b1 >= 0) { p += 2u + (uint32_t)b1; return true; }
+  uint32_t q = p + 1, el;
+  if (!t_len(t, q, end, el)) return false;
+  p = q + el;
+  return true;
+}
 
 // l bytes of the tile -> global memory at any alignment: bytes up to the first aligned word, whole words, tail bytes.  The
 // 32 lanes of a warp copy the cells of 32 consecutive rows, which are adjacent in the output: the partial lines merge in L2.
@@ -250,15 +267,22 @@ __device__ __forceinline__ uint32_t crc_chunks(const uint32_t* g, const Tile& t,
 }
 
 // shared memory layout (dynamic), all sections 16-byte aligned:
-//   [0,16) mbarrier | CRC tables g5 2 KiB + xp16 2 KiB | seen words [32][4] u32 + CRC accumulators [32] | DevField[nf] | FieldTemplate[nf] | names | tile bytes
-// Everything between the mbarrier and the tile is constant per schema ("consts": built once per decoder in this layout,
-// api.cu) and arrives with ONE bulk copy on the same mbarrier as the tile.
+//   [0,16) mbarrier | CRC tables g5 2 KiB + xp16 2 KiB | seen words [32][4] u32 + CRC accumulators [32] | DevField[nf] | FieldTemplate[nf] | names | entry table | tile bytes
+// Everything between the mbarrier and the entry table is constant per schema ("consts": built once per decoder in this
+// layout, api.cu) and arrives with ONE bulk copy on the same mbarrier as the tile.
 #define TILE_SEEN_BYTES (512u + 128u + 16u) // seen words [32][4], the CRC accumulators [32], then the mask of rows some warp gave up on; zero in the consts blob
 #define TILE_CRC_BYTES (2048u + 2048u)     // g5, xp16
 __host__ __device__ inline uint32_t tile_schema_smem(uint32_t nf, uint32_t names_bytes) {
   return ((nf * (uint32_t)sizeof(DevField) + 15u) & ~15u) + ((nf * (uint32_t)sizeof(FieldTemplate) + 15u) & ~15u) + ((names_bytes + 15u) & ~15u);
 }
 __host__ __device__ inline uint32_t tile_const_bytes(uint32_t nf, uint32_t names_bytes) { return TILE_CRC_BYTES + TILE_SEEN_BYTES + tile_schema_smem(nf, names_bytes); }
+// entry table of the Example features / SequenceExample context: where map entry e of record `lane` starts, as a u16 offset
+// from the record's payload, at [e][lane] (a warp reading one row touches 64 consecutive bytes: no bank conflict); then per
+// lane the number of entries [32] and how many of them the table holds [32] u32.  One row per schema field: a record the
+// fast path takes has at most one entry per field it reads, and entries beyond (fields the reader prunes) are hopped to.
+// Only the 12 + 3 warp kernels build it; the sizing counts it for every tile (small schemas: a few hundred bytes).
+__host__ __device__ inline uint32_t tile_entry_rows(uint32_t nf) { return nf; }
+__host__ __device__ inline uint32_t tile_entry_bytes(uint32_t nf) { return tile_entry_rows(nf) * 32u * 2u + 256u; }
 // ragged mode scratch behind the tile: cell source offsets [n_var][32] | per-array counts -> local offsets [n_cnt][32] | totals [n_cnt] | bases u64 [n_cnt] | tile id
 __host__ __device__ inline uint32_t tile_ragged_bytes(uint32_t n_var, uint32_t n_cnt) { return (n_var + n_cnt) * 128u + n_cnt * 4u + n_cnt * 8u + 16u + 16u + 96u; }
 #define TILE_SQ_STEPS 128u       // FeatureList steps per record the one-pass mode keeps per-step element counts for
@@ -266,13 +290,13 @@ __host__ __device__ inline uint32_t tile_ragged_bytes(uint32_t n_var, uint32_t n
 // the per-step element counts [n_var][TILE_SQ_STEPS][32] u8
 __host__ __device__ inline uint32_t tile_seq_bytes(uint32_t n_var, bool with_steps = false) { return n_var * 256u + 16u + (with_steps ? n_var * TILE_SQ_STEPS * 32u : 0u); }
 __host__ __device__ inline uint32_t tile_smem_bytes(uint32_t nf, uint32_t names_bytes, uint32_t tile_cap, uint32_t ragged_bytes = 0) {
-  return 16 + tile_const_bytes(nf, names_bytes) + tile_cap + 64 + ragged_bytes;   // +64: template compares may look a few bytes past the tile
+  return 16 + tile_const_bytes(nf, names_bytes) + tile_entry_bytes(nf) + tile_cap + 64 + ragged_bytes;   // +64: template compares may look a few bytes past the tile
 }
 
 // PW parse warps + CW CRC warps per tile.  Large records: shared memory allows three tiles per SM, so a tile gets 12 + 3 warps
 // (45 resident warps).  Small records: a tile is a few KB, eight fit an SM, and 4 + 1 warps per tile give the same number of
 // resident warps with three times as many records in flight (a tile's life is a latency chain: offsets -> bulk copy -> parse
-// -> barriers -> stores) and a third of the hops (every parse warp walks every entry).
+// -> entry walk -> parse -> barriers -> stores).
 // XC: the kernel can re-encode malformed UTF-8 strings of ragged columns itself (calls into the out-of-line Java transcoder).
 // Merely containing those calls slows the kernel down (registers and code size, even when they never execute), so the
 // default instantiation has none: it raises TF_XCODE instead and the host re-runs the batch -- and the next ones -- with XC.
@@ -287,7 +311,9 @@ __global__ void __launch_bounds__((PW + CW) * 32, (PW >= 16 ? 2 : PW >= 12 ? TIL
   DevField* sfields = reinterpret_cast<DevField*>(sbase);
   FieldTemplate* stpl = reinterpret_cast<FieldTemplate*>(sbase + ((nf * (uint32_t)sizeof(DevField) + 15u) & ~15u));
   uint8_t* snames = sbase + ((nf * (uint32_t)sizeof(DevField) + 15u) & ~15u) + ((nf * (uint32_t)sizeof(FieldTemplate) + 15u) & ~15u);
-  uint8_t* tile_b = sbase + tile_schema_smem(nf, A.names_bytes);
+  uint16_t* eoff = reinterpret_cast<uint16_t*>(sbase + tile_schema_smem(nf, A.names_bytes));    // entry table [E][32] (see tile_entry_bytes)
+  uint32_t* ecnt = reinterpret_cast<uint32_t*>(eoff + tile_entry_rows(nf) * 32u);              // [32] entries, [32] entries in the table
+  uint8_t* tile_b = sbase + tile_schema_smem(nf, A.names_bytes) + tile_entry_bytes(nf);
   const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;                          // warps 0..W-1 parse, warp W = CRC
 
   // Record r of the tile is copied to its place in the tile: bytes [off_r & ~15, off_r + framed length) -> tile + rbase_r.
@@ -443,13 +469,13 @@ __global__ void __launch_bounds__((PW + CW) * 32, (PW >= 16 ? 2 : PW >= 12 ? TIL
 
   // =============================== warps 0..W-1: parse ===============================
   bool bad = false;
-  uint32_t skip = wid;                     // entries to hop before the next one this warp owns (entry index % W == wid)
   uint32_t shape_bad = 0;
   unsigned long long seen_lo = 0, seen_hi = 0;
+  uint32_t p = pay;
+  uint32_t cend = end, fl_start = end, fl_end = end;        // context/features region = [p, cend), feature_lists = [fl_start, fl_end)
   if (active) {
-    uint32_t p = pay, L = 0;
-    uint32_t cend = end, fl_start = end, fl_end = end;      // context/features region = [p, cend), feature_lists = [fl_start, fl_end)
     // Example { features = 1 } / SequenceExample { context = 1, feature_lists = 2 }: exactly these fields, in this order
+    uint32_t L = 0;
     if (len < 2 || T.u8(p) != 0x0A) bad = true;
     else {
       ++p;
@@ -462,28 +488,55 @@ __global__ void __launch_bounds__((PW + CW) * 32, (PW >= 16 ? 2 : PW >= 12 ? TIL
         else { ++q; if (!t_len(T, q, end, L2) || q + L2 != end) bad = true; else { fl_start = q; fl_end = end; } }
       }
     }
-    uint32_t next_f = wid;                 // in-order data: this warp's k-th owned entry is field wid + k*W
-    while (!bad && p < cend) {
-      // hop over the entries the other parse warps own (`0A elen ...`): a tight loop, one byte load + add per entry.
-      // The owner validates those entries; p + 1 <= cend is always inside the tile and an overshoot is caught by the
-      // p == cend check after the loop.
-      for (bool wide = true; wide;) {
-        wide = false;
-        while (skip && p < cend) {                           // the tight part: single-byte entry lengths only
-          const int32_t b1 = T.i8(p + 1);
-          if (b1 < 0) { wide = true; break; }
-          p += 2u + (uint32_t)b1;
-          --skip;
-        }
-        if (wide) {                                          // an entry of 128+ bytes: full length varint, then back to the loop
-          uint32_t q = p + 1, el;
-          if (!t_len(T, q, cend, el)) { bad = true; break; }
-          p = q + el;
-          --skip;
-        }
+  }
+  // 12 + 3 warps (TABLE): the last parse warp (it owns the fewest entries) builds the entry table, the parse warps wait for
+  // it at the barrier and then take every entry from the table.  4 + 1 warps: small records, where a tile's life is a
+  // latency chain and a walk in front of the barrier lengthens it (measured: the 220-byte string records lost 1.5 %, and
+  // 3.5 % when the other warps parsed their first entry during the walk): each warp hops from its last entry to its next
+  // one (PW - 1 hops) and checks that the chain ends exactly on cend.
+  constexpr bool TABLE = PW >= 12;
+  constexpr uint32_t walker = PW - 1;
+  if (TABLE && wid == walker) {
+    // ---- the entry table: ONE walk of the record's `0A elen` chain, which must end exactly on cend (the owners validate
+    //      the entries themselves).  A broken chain is recorded as ~0 entries: every parse warp gives the row up. ----
+    const uint32_t rows_e = tile_entry_rows(nf);
+    uint32_t ne = 0, ni = 0;
+    if (active && !bad) {
+      uint32_t q = p;
+      while (q < cend) {
+        if (ne < rows_e && q - pay <= 0xffffu) { eoff[ne * 32u + lane] = (uint16_t)(q - pay); ni = ne + 1; }
+        if (!t_next_entry(T, q, cend)) break;
+        ++ne;
       }
-      if (bad || p >= cend) break;
-      skip = PW - 1;                           // this entry is ours; W - 1 hops to the next
+      if (q != cend) ne = ~0u;
+    }
+    ecnt[lane] = ne;
+    ecnt[32 + lane] = ni;
+  }
+  uint32_t skip = 0;                       // SequenceExample: feature_lists entries to pass before the next one this warp owns
+  uint32_t i = wid;                        // the next entry this warp owns (entry index % W == wid)
+  uint32_t next_f = wid;                   // in-order data: this warp's k-th owned entry is field wid + k*W
+#pragma unroll 1
+  for (uint32_t phase = TABLE ? 1u : 0u; phase < (TABLE ? 2u : 1u); ++phase) {     // 0: by hopping (4 + 1 warps); 1: from the table
+    if (phase) {
+      __syncwarp();                                  // (the lanes of a warp arrive together)
+      asm volatile("bar.sync 1, %0;" ::"r"(PW * 32) : "memory");
+      if (active && ecnt[lane] == ~0u) bad = true;
+    }
+    if (!active) continue;
+    while (!bad && i < (phase ? ecnt[lane] : ~0u)) {
+      const uint32_t n_idx = phase ? ecnt[32 + lane] : 0u;   // entries in the table
+      if (i < n_idx) p = pay + eoff[i * 32u + lane];
+      else {
+        // not in the table: hop on from the later of this warp's position (p: the start of the entry after its last one,
+        // or of entry 0) and the table's last entry.  Without the table the chain is checked here: a hop that reaches cend
+        // means there is no such entry, and the chain must end exactly there (below).
+        uint32_t at = i >= PW ? i - (PW - 1) : 0u;
+        if (at + 1 < n_idx) { at = n_idx - 1; p = pay + eoff[at * 32u + lane]; }
+        for (; at < i && p < cend; ++at) if (!t_next_entry(T, p, cend)) { bad = true; break; }
+        if (bad || p >= cend) break;
+      }
+      i += PW;
       // ---- owned entry: try the expected field's template first ----
       uint32_t eend, kind, llen;
       int f = -1;
@@ -733,7 +786,10 @@ __global__ void __launch_bounds__((PW + CW) * 32, (PW >= 16 ? 2 : PW >= 12 ? TIL
       }
       p = eend;
     }
-    if (p != cend) bad = true;
+    if (!TABLE && p != cend) bad = true;
+  }
+  if (active) {
+    if (TABLE) skip = i - ecnt[lane];
     // ---- SequenceExample.feature_lists: { 0A elen 0A klen key 12 vlen FeatureList }*, FeatureList = { 0A flen Feature }* ----
     // A SequenceExample typically has few FeatureLists with many steps each: handing whole entries to warps would leave most
     // of the tile's warps idle behind the one that walks a 64-step list.  Every parse warp therefore walks EVERY entry's
