@@ -235,6 +235,42 @@ void    tfr_encoder_destroy(tfr_encoder*);
  * TFR_E_NULL_IN_NONNULL with *error_row set.                                               */
 int32_t tfr_encode(tfr_encoder*, const tfr_column* columns, int32_t n, int32_t columns_on_device,
                    void** out_dev, size_t* out_bytes, int64_t* error_row);
+/* ---- encode from Spark UnsafeRows ------------------------------------------------------
+ * What OutputWriter.write(row: InternalRow) receives is an UnsafeRow (plan output and
+ * FileFormatWriter's partition projection both are), so the JVM side only appends each row's
+ * bytes (one Platform.copyMemory) and its offset; the GPU takes the rows apart.
+ *
+ * Input layout (Spark's published UnsafeRow / UnsafeArrayData format; all words little-endian):
+ *   row    : null bitset of ((nf + 63) / 64) 64-bit words (bit i set = field i is null), then
+ *            one 8-byte slot per field, then the variable-length region.
+ *   slots  : IntegerType, FloatType: the low 4 bytes.  LongType, DoubleType: all 8 bytes.
+ *            DecimalType: the 8 bytes as a signed unscaled long.  StringType, BinaryType and
+ *            arrays: (offset << 32) | size, offset relative to the row start.
+ *   array  : int64 numElements n; element null bitset of ((n + 63) / 64) words; the elements,
+ *            padded to 8 bytes (4 bytes each for int and float, 8 for long, double and decimal;
+ *            string, binary and inner-array elements are 8-byte (offset << 32) | size slots with
+ *            offset relative to the array start); then the variable-length region.
+ *   batch  : row r is rows[row_offsets[r] .. row_offsets[r+1]); row_offsets has n_rows + 1
+ *            int32 entries, multiples of 8, non-decreasing.  rows and row_offsets are both host
+ *            memory (pageable or the staging below) or both device memory (on_device != 0); any
+ *            8-byte aligned rows pointer works.  A batch stays below 2 GiB.
+ *
+ * Semantics: the framed bytes tfr_encode produces for the same rows given as columns, plus
+ *   - a null field is omitted; in a non-nullable field (NullType included): TFR_E_NULL_IN_NONNULL;
+ *   - DecimalType v: FloatList value (float)v, round to nearest even (BigDecimal(v, 0).floatValue,
+ *     M/TFRecordSerializer.scala:88-90,170-171);
+ *   - a null element of an int, long, float or double array: the slot's bits (toXArray copies
+ *     them, :103-113; Spark writes 0);
+ *   - a null element of a string, binary or decimal array, or a null inner array of a 2-D
+ *     column: TFR_E_NULL_IN_NONNULL (:118-135,141-142);
+ *   - a malformed row (a slot or element offset/size outside its row or array, a row shorter
+ *     than its fixed region, a negative or oversized numElements, a misaligned offset):
+ *     TFR_E_INVALID_ARG.  No byte outside rows[row_offsets[0] .. row_offsets[n_rows]) is read.
+ *   *error_row is the first failing row; a row that fails both ways is TFR_E_INVALID_ARG.
+ * The result is read like tfr_encode's (*out_dev, tfr_encoder_result_host).                  */
+int32_t tfr_encoder_row_staging(tfr_encoder*, size_t min_bytes, void** host_ptr, size_t* capacity);
+int32_t tfr_encode_rows(tfr_encoder*, const void* rows, const int32_t* row_offsets, int64_t n_rows,
+                        int32_t on_device, void** out_dev, size_t* out_bytes, int64_t* error_row);
 /* copy the last encode result to host memory (pinned staging owned by the encoder) */
 int32_t tfr_encoder_result_host(tfr_encoder*, void** host_ptr, size_t* nbytes);
 int32_t tfr_encoder_stream(tfr_encoder*, void** cuda_stream);

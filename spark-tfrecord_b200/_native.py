@@ -25,7 +25,8 @@ EXPORTS = [
     "tfr_decoder_num_staging_slots", "tfr_decode", "tfr_decode_submit",
     "tfr_decoder_stream", "tfr_decoder_set_profiling", "tfr_decoder_get_profile", "tfr_decoder_get_stats", "tfr_batch_wait", "tfr_batch_status", "tfr_batch_consumed", "tfr_batch_num_columns", "tfr_batch_columns",
     "tfr_batch_to_host_async", "tfr_batch_to_host", "tfr_batch_export_arrow_host", "tfr_batch_export_arrow_device", "tfr_batch_release",
-    "tfr_encoder_create", "tfr_encoder_destroy", "tfr_encode", "tfr_encoder_result_host", "tfr_encoder_stream",
+    "tfr_encoder_create", "tfr_encoder_destroy", "tfr_encode", "tfr_encoder_row_staging", "tfr_encode_rows", "tfr_encoder_result_host",
+    "tfr_encoder_stream",
     "tfr_infer_create", "tfr_infer_update", "tfr_infer_update_block", "tfr_infer_result", "tfr_infer_name", "tfr_infer_destroy",
 ]
 
@@ -126,6 +127,8 @@ def lib():
         "tfr_encoder_create": (i32, [vp, i32, u32, P(vp)]),
         "tfr_encoder_destroy": (None, [vp]),
         "tfr_encode": (i32, [vp, P(tfr_column), i32, i32, P(vp), P(sz), P(i64)]),
+        "tfr_encoder_row_staging": (i32, [vp, sz, P(vp), P(sz)]),
+        "tfr_encode_rows": (i32, [vp, vp, vp, i64, i32, P(vp), P(sz), P(i64)]),
         "tfr_encoder_result_host": (i32, [vp, P(vp), P(sz)]),
         "tfr_encoder_stream": (i32, [vp, P(vp)]),
         "tfr_infer_create": (i32, [i32, i32, P(vp)]),
@@ -368,6 +371,39 @@ class Encoder:
         cols = [c.to_ctypes() for c in columns]
         self.encode_columns(cols, False)
         return self.result_host()
+
+    def row_staging(self, nbytes: int) -> np.ndarray:
+        """pinned host memory for UnsafeRow bytes (tfr_encoder_row_staging); valid until a call that needs more"""
+        p = C.c_void_p()
+        cap = C.c_size_t()
+        _check(lib().tfr_encoder_row_staging(self.h, nbytes, C.byref(p), C.byref(cap)))
+        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=(cap.value,))
+
+    def encode_rows(self, rows, offsets, on_device: Optional[bool] = None):
+        """Spark UnsafeRows -> (device ptr, nbytes) of the framed records (tfr_encode_rows).  rows: the row bytes, offsets:
+        n_rows + 1 int32 row starts; numpy / bytes (host) or torch tensors (host or CUDA).  Raises TfrError with code
+        TFR_E_INVALID_ARG for a malformed row and NullPointerException for a null the writer cannot take; .row is the row."""
+        rp, _, rdev, keep_r = _device_ptr(rows)
+        if not isinstance(offsets, tuple):
+            try:
+                import torch
+                is_t = isinstance(offsets, torch.Tensor)
+            except ImportError:
+                is_t = False
+            offsets = offsets.to(torch.int32) if is_t else np.asarray(offsets, dtype=np.int32)
+        op, onb, odev, keep_o = _device_ptr(offsets)
+        if rdev != odev:
+            raise ValueError("rows and offsets must both be host or both be device memory")
+        n_rows = onb // 4 - 1 if not isinstance(offsets, tuple) else offsets[1] // 4 - 1
+        dev = rdev if on_device is None else (1 if on_device else 0)
+        out = C.c_void_p()
+        nb = C.c_size_t()
+        er = C.c_int64(-1)
+        rc = lib().tfr_encode_rows(self.h, rp, op, max(n_rows, 0), dev, C.byref(out), C.byref(nb), C.byref(er))
+        if rc != 0:
+            msg = lib().tfr_last_error()
+            raise error_for(rc, msg.decode("utf-8", "replace") if msg else "", er.value)
+        return out.value or 0, nb.value
 
     def result_host(self) -> bytes:
         p = C.c_void_p()

@@ -23,6 +23,7 @@
 #include "frame.cuh"
 #include "host_util.h"
 #include "infer.cuh"
+#include "rows.cuh"
 #include "scan.cuh"
 #include "tile.cuh"
 

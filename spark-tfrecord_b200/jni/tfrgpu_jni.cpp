@@ -21,6 +21,8 @@
 //     static native long encoderCreate(long schema, int device);
 //     static native void encoderDestroy(long encoder);    // OutputWriter.close (M/TFRecordOutputWriter.scala:40-43)
 //     static native java.nio.ByteBuffer encode(long encoder, long[] columnStructAddrs, int n);   // framed bytes, pinned
+//     static native java.nio.ByteBuffer encoderRowStaging(long encoder, long minBytes);          // direct, pinned: UnsafeRow bytes
+//     static native java.nio.ByteBuffer encodeRows(long encoder, java.nio.ByteBuffer rows, java.nio.ByteBuffer offsets, int nRows);
 //     static native long inferCreate(int recordType, int device);                                 // DefaultSource.inferSchema (M/DefaultSource.scala:31-39)
 //     static native long inferUpdate(long infer, java.nio.ByteBuffer block, long nbytes, boolean isFinal);   // -> consumed bytes
 //     static native Object[] inferResult(long infer);     // {String[] names (bytewise sorted), int[] lattice codes}
@@ -178,6 +180,31 @@ extern "C" JNIEXPORT jobject JNICALL Java_com_linkedin_spark_datasources_tfrecor
   rc = tfr_encoder_result_host((tfr_encoder*)enc, &host, &nb);
   if (rc) { throw_for(env, rc, -1); return nullptr; }
   return env->NewDirectByteBuffer(host, (jlong)nb);          // outputStream.write(...) of these bytes == the reference file
+}
+// Row path (INTEGRATION.md): write(row) copies the UnsafeRow's bytes into this pinned buffer and appends its offset
+extern "C" JNIEXPORT jobject JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_encoderRowStaging(JNIEnv* env, jclass, jlong enc, jlong minBytes) {
+  void* p = nullptr; size_t cap = 0;
+  int32_t rc = tfr_encoder_row_staging((tfr_encoder*)enc, (size_t)minBytes, &p, &cap);
+  if (rc) { throw_for(env, rc, -1); return nullptr; }
+  return env->NewDirectByteBuffer(p, (jlong)cap);
+}
+// rows: the staging buffer; offsets: a direct buffer of nRows + 1 int32 row starts.  A malformed row throws
+// IllegalArgumentException, a null the reference cannot write NullPointerException, both with the row.
+extern "C" JNIEXPORT jobject JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_encodeRows(JNIEnv* env, jclass, jlong enc, jobject rows,
+                                                                                                 jobject offsets, jint nRows) {
+  void* dev = nullptr; size_t nb = 0; int64_t err_row = -1;
+  int32_t rc = tfr_encode_rows((tfr_encoder*)enc, env->GetDirectBufferAddress(rows), (const int32_t*)env->GetDirectBufferAddress(offsets),
+                               (int64_t)nRows, 0, &dev, &nb, &err_row);
+  if (rc == TFR_E_INVALID_ARG) {
+    std::string msg = "malformed UnsafeRow" + (err_row >= 0 ? " (row " + std::to_string(err_row) + ")" : std::string()) + ": " + tfr_last_error();
+    env->ThrowNew(env->FindClass("java/lang/IllegalArgumentException"), msg.c_str());
+    return nullptr;
+  }
+  if (rc) { throw_for(env, rc, err_row); return nullptr; }
+  void* host = nullptr;
+  rc = tfr_encoder_result_host((tfr_encoder*)enc, &host, &nb);
+  if (rc) { throw_for(env, rc, -1); return nullptr; }
+  return env->NewDirectByteBuffer(host, (jlong)nb);
 }
 
 // ---- schema inference: DefaultSource.inferSchema -> TensorFlowInferSchema (M/DefaultSource.scala:31-39,48-70) ----
