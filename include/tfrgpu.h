@@ -155,7 +155,8 @@ int32_t tfr_decoder_stream(tfr_decoder*, void** cuda_stream /* cudaStream_t */);
  *   ms[0] frame index (scan+check+repair+finish+emit)   ms[1] decode pass 1 (CRC + parse)
  *   ms[2] scans + summary                               ms[3] decode pass 2 (variable-width emit)
  *   ms[4] validity pack                                 ms[5] H2D of the input (host input only)
- *   ms[6] D2H of the Arrow buffers (tfr_batch_to_host[_async])
+ *   ms[6] D2H of the Arrow buffers (tfr_batch_to_host[_async]) or of the rows (tfr_batch_rows)
+ *   ms[7] the rows pass of tfr_batch_rows (size kernel, scan, emit kernel)
  * plus the number of kernel launches and of pass-1 launches.                                  */
 #define TFR_PROFILE_STAGES 8
 int32_t tfr_decoder_set_profiling(tfr_decoder*, int32_t enable);
@@ -220,6 +221,42 @@ int32_t tfr_batch_to_host(tfr_batch*, tfr_column* out, int32_t n);
 int32_t tfr_batch_export_arrow_host(tfr_batch*, int32_t column, void* arrow_array, void* arrow_schema);
 int32_t tfr_batch_export_arrow_device(tfr_batch*, int32_t column, void* arrow_device_array, void* arrow_schema);
 void    tfr_batch_release(tfr_batch*);
+
+/* ---- decode to Spark UnsafeRows ---------------------------------------------------------
+ * What a row-based FileFormat reader returns is an Iterator[InternalRow] (M/DefaultSource.scala:129-135), which Spark
+ * turns into UnsafeRows with an UnsafeProjection, field by field on the JVM.  tfr_batch_rows lays the batch's rows out in
+ * that format on the GPU, so the JVM side only points one reused UnsafeRow at each row (INTEGRATION.md).
+ *
+ * The batch's rows (the n_rows rows before its first error, tfr_batch_info.n_rows) as Spark UnsafeRows, back to back:
+ * row r is rows[row_offsets[r] .. row_offsets[r+1]).  to_host = 0: device memory; 1: pinned host memory.  row_offsets
+ * has n_rows + 1 int64 entries, offsets[0] = 0, every entry a multiple of 8 (the rows of one batch can exceed 2 GiB even
+ * though its framed bytes cannot: an empty string is 2 bytes of protobuf and 8 of row).  Owned by the batch and valid
+ * until tfr_batch_release; a second call returns the same buffers (to_host = 1 after 0 adds only the copy).  Waits for
+ * the batch like tfr_batch_to_host, and returns when the rows (and their copy) are complete.  An empty batch gives
+ * n_rows = 0, offsets = {0}, nbytes = 0.
+ *
+ * Output layout (the one tfr_encode_rows reads above): what Spark's UnsafeProjection makes of the SpecificInternalRow
+ * the reference's deserializer fills (M/TFRecordDeserializer.scala:21-61):
+ *   - a null bitset of (nf + 63) / 64 words, one 8-byte slot per field, then the variable-length region: variable values
+ *     in field order, each 8-byte aligned with zeroed padding; the row size is a multiple of 8;
+ *   - a null field, and every NullType field, has its bit set and a zero slot;
+ *   - IntegerType, FloatType: the low 4 bytes, the high 4 bytes zero.  LongType, DoubleType: all 8 bytes;
+ *   - float and double bits are copied from the decoded columns unchanged (the decoder has already quieted sNaN when
+ *     it widened a float to double): Spark 3.5's UnsafeWriter (Platform.putFloat / putDouble) normalises neither NaN
+ *     nor -0.0.  This rule is restated, not checked against a JVM;
+ *   - StringType, BinaryType: slot (offset << 32) | size from the row start; strings are the Java re-encoded bytes the
+ *     decoder emits;
+ *   - arrays: UnsafeArrayData -- numElements, an all-zero element null bitset (decode never produces a null element),
+ *     the elements padded to 8 bytes (4 bytes each for int and float, 8 for long and double, 8-byte (offset << 32) | size
+ *     slots from the array start for strings, binaries and the inner arrays of 2-D columns), then the array's variable
+ *     region;
+ *   - ByteArray records are one binary field.
+ * Errors: TFR_E_INVALID_ARG (a null batch or output pointer); TFR_E_UNSUPPORTED_TYPE when the schema has a DecimalType
+ * field (its UnsafeRow layout depends on the declared precision and scale, which tfr_field does not carry;
+ * tfr_last_error names the field); TFR_E_BATCH_TOO_LARGE when one row would exceed INT32_MAX bytes
+ * (UnsafeRow.sizeInBytes is an int); TFR_E_OOM / TFR_E_CUDA.                                                            */
+int32_t tfr_batch_rows(tfr_batch*, int32_t to_host, const void** rows, const int64_t** row_offsets,
+                       int64_t* n_rows, size_t* nbytes);
 
 /* ---- encode: replaces TFRecordOutputWriter.write/close -------------------------------- */
 /* Replaces the constructor M/TFRecordOutputWriter.scala:12-24.                             */

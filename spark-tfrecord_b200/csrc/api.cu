@@ -26,6 +26,7 @@
 #include "rows.cuh"
 #include "scan.cuh"
 #include "tile.cuh"
+#include "urows.cuh"
 
 // ---------------------------------------------------------------------------------------------
 // errors

@@ -77,37 +77,50 @@ __global__ void __launch_bounds__(1024) scan_tile_bases_kernel(uint64_t* __restr
   }
 }
 
+// Local scan of tile t of array a into dst (n+1 entries of Out), summing in Acc: uint32_t for int32 Arrow offsets (the
+// totals were checked against int32 by scan_tile_bases_kernel), uint64_t for int64 offsets of totals beyond 4 GiB.
+template <typename Out, typename Acc>
+__device__ __forceinline__ void scan_apply_tile(const uint32_t* __restrict__ cnt, uint32_t n, uint32_t n_tiles, const uint64_t* __restrict__ tbase,
+                                                const uint64_t* __restrict__ totals_raw, Out* dst) {
+  __shared__ Acc wsum[SCAN_THREADS / 32];
+  const uint32_t a = blockIdx.y, t = blockIdx.x, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const uint32_t* src = cnt + (size_t)a * n;
+  // thread owns SCAN_ITEMS consecutive elements
+  uint32_t base = t * SCAN_TILE + threadIdx.x * SCAN_ITEMS;
+  uint32_t v[SCAN_ITEMS];
+  Acc s = 0;
+#pragma unroll
+  for (int i = 0; i < SCAN_ITEMS; ++i) { v[i] = base + i < n ? src[base + i] : 0; s += v[i]; }
+  Acc x = s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { Acc y = __shfl_up_sync(FULLMASK, x, o); if (lane >= (uint32_t)o) x += y; }
+  if (lane == 31) wsum[wid] = x;
+  __syncthreads();
+  if (wid == 0) {
+    Acc w = lane < SCAN_THREADS / 32 ? wsum[lane] : 0;
+#pragma unroll
+    for (int o = 1; o < SCAN_THREADS / 32; o <<= 1) { Acc y = __shfl_up_sync(FULLMASK, w, o); if (lane >= (uint32_t)o) w += y; }
+    if (lane < SCAN_THREADS / 32) wsum[lane] = w;
+  }
+  __syncthreads();
+  Acc run = x - s + (wid ? wsum[wid - 1] : 0) + (Acc)tbase[(size_t)a * n_tiles + t];
+#pragma unroll
+  for (int i = 0; i < SCAN_ITEMS; ++i) {
+    if (base + i < n) dst[base + i] = (Out)run;
+    run += v[i];
+  }
+  if (t == n_tiles - 1 && threadIdx.x == 0) dst[n] = (Out)(Acc)totals_raw[a];
+}
+
 // out[a]: n+1 int32 entries
 __global__ void __launch_bounds__(SCAN_THREADS) scan_apply_kernel(const uint32_t* __restrict__ cnt, uint32_t n, uint32_t n_tiles,
                                                                   const uint64_t* __restrict__ tbase, const uint64_t* __restrict__ totals_raw,
                                                                   int32_t* const* __restrict__ out) {
-  __shared__ uint32_t wsum[SCAN_THREADS / 32];
-  const uint32_t a = blockIdx.y, t = blockIdx.x, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const uint32_t* src = cnt + (size_t)a * n;
-  int32_t* dst = out[a];
-  // thread owns SCAN_ITEMS consecutive elements
-  uint32_t base = t * SCAN_TILE + threadIdx.x * SCAN_ITEMS;
-  uint32_t v[SCAN_ITEMS];
-  uint32_t s = 0;
-#pragma unroll
-  for (int i = 0; i < SCAN_ITEMS; ++i) { v[i] = base + i < n ? src[base + i] : 0; s += v[i]; }
-  uint32_t x = s;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { uint32_t y = __shfl_up_sync(FULLMASK, x, o); if (lane >= (uint32_t)o) x += y; }
-  if (lane == 31) wsum[wid] = x;
-  __syncthreads();
-  if (wid == 0) {
-    uint32_t w = lane < SCAN_THREADS / 32 ? wsum[lane] : 0;
-#pragma unroll
-    for (int o = 1; o < SCAN_THREADS / 32; o <<= 1) { uint32_t y = __shfl_up_sync(FULLMASK, w, o); if (lane >= (uint32_t)o) w += y; }
-    if (lane < SCAN_THREADS / 32) wsum[lane] = w;
-  }
-  __syncthreads();
-  uint32_t run = x - s + (wid ? wsum[wid - 1] : 0) + (uint32_t)tbase[(size_t)a * n_tiles + t];
-#pragma unroll
-  for (int i = 0; i < SCAN_ITEMS; ++i) {
-    if (base + i < n) dst[base + i] = (int32_t)run;
-    run += v[i];
-  }
-  if (t == n_tiles - 1 && threadIdx.x == 0) dst[n] = (int32_t)(uint32_t)totals_raw[a];
+  scan_apply_tile<int32_t, uint32_t>(cnt, n, n_tiles, tbase, totals_raw, out[blockIdx.y]);
+}
+// out: n+1 int64 entries (one array)
+__global__ void __launch_bounds__(SCAN_THREADS) scan_apply64_kernel(const uint32_t* __restrict__ cnt, uint32_t n, uint32_t n_tiles,
+                                                                    const uint64_t* __restrict__ tbase, const uint64_t* __restrict__ totals_raw,
+                                                                    int64_t* __restrict__ out) {
+  scan_apply_tile<int64_t, uint64_t>(cnt, n, n_tiles, tbase, totals_raw, out);
 }

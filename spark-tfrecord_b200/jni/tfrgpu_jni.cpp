@@ -18,6 +18,7 @@
 //     static native void batchExportArrowDevice(long batch, int column, long arrowDeviceArrayAddr, long arrowSchemaAddr);  // ColumnarBatch on the GPU (spark-rapids)
 //     static native void batchThrowIfError(long batch);   // the exception the reference would throw for the first failing record
 //     static native void batchRelease(long batch);
+//     static native java.nio.ByteBuffer[] batchRows(long batch);   // {rows, int64 row offsets}: pinned UnsafeRows, valid until batchRelease
 //     static native long encoderCreate(long schema, int device);
 //     static native void encoderDestroy(long encoder);    // OutputWriter.close (M/TFRecordOutputWriter.scala:40-43)
 //     static native java.nio.ByteBuffer encode(long encoder, long[] columnStructAddrs, int n);   // framed bytes, pinned
@@ -158,6 +159,17 @@ extern "C" JNIEXPORT void JNICALL Java_com_linkedin_spark_datasources_tfrecord_T
   if (rc == 0 && i.error_code == 0) return;
   tfr_batch_release((tfr_batch*)batch);
   throw_for(env, rc ? rc : i.error_code, rc ? -1 : i.error_row);
+}
+// The rows of a batch as UnsafeRows in pinned memory: the iterator points one reused UnsafeRow at row i with
+// pointTo(null, address(rows) + off(i), (int)(off(i + 1) - off(i))) -- no per-field work on the JVM.
+extern "C" JNIEXPORT jobjectArray JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_batchRows(JNIEnv* env, jclass, jlong batch) {
+  const void* rows = nullptr; const int64_t* offs = nullptr; int64_t n = 0; size_t nb = 0;
+  int32_t rc = tfr_batch_rows((tfr_batch*)batch, 1, &rows, &offs, &n, &nb);
+  if (rc) { throw_for(env, rc, -1); return nullptr; }         // a decimal schema keeps the column views; the batch stays usable
+  jobjectArray out = env->NewObjectArray(2, env->FindClass("java/nio/ByteBuffer"), nullptr);
+  env->SetObjectArrayElement(out, 0, env->NewDirectByteBuffer(const_cast<void*>(rows), (jlong)nb));
+  env->SetObjectArrayElement(out, 1, env->NewDirectByteBuffer(const_cast<int64_t*>(offs), (jlong)((n + 1) * 8)));
+  return out;
 }
 extern "C" JNIEXPORT void JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_batchRelease(JNIEnv*, jclass, jlong batch) { if (batch) tfr_batch_release((tfr_batch*)batch); }
 extern "C" JNIEXPORT void JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_encoderDestroy(JNIEnv*, jclass, jlong enc) { if (enc) tfr_encoder_destroy((tfr_encoder*)enc); }
