@@ -258,6 +258,43 @@ void    tfr_batch_release(tfr_batch*);
 int32_t tfr_batch_rows(tfr_batch*, int32_t to_host, const void** rows, const int64_t** row_offsets,
                        int64_t* n_rows, size_t* nbytes);
 
+/* The same rows with a file's partition values appended: what Spark's FileFormat.buildReaderWithPartitionValues makes of
+ * each row, UnsafeProjection (GenerateUnsafeProjection) over D ++ P of JoinedRow(dataRow, file.partitionValues), where D
+ * is the decoder's schema (nd fields) and P the partition schema (np = n_part_fields fields).  tfr_batch_rows is this
+ * call with np = 0, and its output is the layout above.  Row layout:
+ *   - a null bitset of (nd + np + 63) / 64 words: data field i is bit i, partition field j is bit nd + j;
+ *   - nd + np slots, the data fields' then the partition fields';
+ *   - the data fields' variable region, laid out as above after this larger fixed region;
+ *   - then the partition row's variable region, unchanged.
+ * part_row is the partition values as an UnsafeRow of P alone (UnsafeProjection.create(partitionSchema) applied to
+ * file.partitionValues, once per file): host memory of any alignment, part_row_bytes long, copied during the call.
+ * part_var[j] = 1 when partition slot j is (offset << 32) | size: StringType, BinaryType and DecimalType with precision
+ * > 18; 0 for every other type, whose slot is copied as 8 opaque bytes (Boolean, Byte, Short, Integer, Long, Float,
+ * Double, Date, Timestamp, Decimal with precision <= 18).  The GPU does not interpret the partition row: it ORs its null
+ * bit j into bit nd + j, copies its slots, and copies its variable region (part_row_bytes - 8 * ((np + 63) / 64 + np)
+ * bytes) to the end of each row.  A flagged slot whose 8 bytes are nonzero gets its offset moved to the region's place
+ * in that row; a zero slot stays zero.  That rule is exact for the rows Spark's UnsafeRowWriter writes, restated here
+ * and NOT checked against a JVM (unpinned, like the float-bits rule above):
+ *   - a null string or binary has its bit set and a zero slot (setNullAt);
+ *   - a null decimal with precision > 18 has its bit set, slot (offset << 32) | 0 and 16 reserved zero bytes in the
+ *     variable region (the generated projection calls write(i, (Decimal) null, precision, scale));
+ *   - a non-null decimal with precision > 18 reserves 16 zero bytes and writes BigInteger.toByteArray() (big-endian,
+ *     minimal two's complement) at their start, its slot holding that length;
+ *   - a non-null value, even an empty one, has an offset of at least 8 (past the null bitset), so its slot is nonzero;
+ *   - Boolean, Byte and Short zero the slot and write 1 or 2 bytes; Date is an int of days, Timestamp a long of
+ *     microseconds; a decimal with precision <= 18 puts its unscaled long in the slot.
+ * With nd = 0 (SELECT of partition columns only, count(*)) every row equals part_row.
+ * A batch's rows are built once: a later call must pass the same partition row (the same bytes, np and flags, nonzero
+ * flags counting as 1; tfr_batch_rows counts as np = 0), or it gets TFR_E_INVALID_ARG and the batch stays usable.
+ * TFR_E_INVALID_ARG, checked before any work and naming the partition field where there is one: n_part_fields outside
+ * 0..4096; part_row or part_var null while np > 0; part_row_bytes not a multiple of 8, smaller than the fixed region
+ * 8 * ((np + 63) / 64 + np), or nonzero while np = 0; a null bit set at an index >= np; a nonzero flagged slot whose
+ * offset is not 8-aligned, lies inside the fixed region, or whose offset + size exceeds part_row_bytes.  The other errors
+ * are tfr_batch_rows' (a DecimalType data field; TFR_E_BATCH_TOO_LARGE counts the partition bytes).                   */
+int32_t tfr_batch_rows_with_partition(tfr_batch*, int32_t to_host, const void* part_row, size_t part_row_bytes,
+                                      int32_t n_part_fields, const uint8_t* part_var, const void** rows,
+                                      const int64_t** row_offsets, int64_t* n_rows, size_t* nbytes);
+
 /* ---- encode: replaces TFRecordOutputWriter.write/close -------------------------------- */
 /* Replaces the constructor M/TFRecordOutputWriter.scala:12-24.                             */
 int32_t tfr_encoder_create(const tfr_schema*, int32_t device, uint32_t flags, tfr_encoder** out);

@@ -25,7 +25,7 @@ EXPORTS = [
     "tfr_decoder_num_staging_slots", "tfr_decode", "tfr_decode_submit",
     "tfr_decoder_stream", "tfr_decoder_set_profiling", "tfr_decoder_get_profile", "tfr_decoder_get_stats", "tfr_batch_wait", "tfr_batch_status", "tfr_batch_consumed", "tfr_batch_num_columns", "tfr_batch_columns",
     "tfr_batch_to_host_async", "tfr_batch_to_host", "tfr_batch_export_arrow_host", "tfr_batch_export_arrow_device", "tfr_batch_release",
-    "tfr_batch_rows",
+    "tfr_batch_rows", "tfr_batch_rows_with_partition",
     "tfr_encoder_create", "tfr_encoder_destroy", "tfr_encode", "tfr_encoder_row_staging", "tfr_encode_rows", "tfr_encoder_result_host",
     "tfr_encoder_stream",
     "tfr_infer_create", "tfr_infer_update", "tfr_infer_update_block", "tfr_infer_result", "tfr_infer_name", "tfr_infer_destroy",
@@ -126,6 +126,7 @@ def lib():
         "tfr_batch_export_arrow_device": (i32, [vp, i32, vp, vp]),
         "tfr_batch_release": (None, [vp]),
         "tfr_batch_rows": (i32, [vp, i32, P(vp), P(vp), P(i64), P(sz)]),
+        "tfr_batch_rows_with_partition": (i32, [vp, i32, vp, sz, i32, vp, P(vp), P(vp), P(i64), P(sz)]),
         "tfr_encoder_create": (i32, [vp, i32, u32, P(vp)]),
         "tfr_encoder_destroy": (None, [vp]),
         "tfr_encode": (i32, [vp, P(tfr_column), i32, i32, P(vp), P(sz), P(i64)]),
@@ -255,13 +256,21 @@ class Batch:
             out.append(pa.Array._import_from_c(int(ffi.cast("uintptr_t", ca)), int(ffi.cast("uintptr_t", cs))))
         return out
 
-    def unsafe_rows(self, to_host: bool = True):
+    def unsafe_rows(self, to_host: bool = True, partition=None):
         """The batch's rows as Spark UnsafeRows (tfr_batch_rows).  to_host=True: (uint8 rows, int64 offsets[n_rows + 1]),
         numpy views of pinned memory the batch owns (valid until release).  to_host=False: (rows device ptr, offsets device
-        ptr, n_rows, nbytes).  Raises UnsupportedTypeException for a schema with a DecimalType field."""
+        ptr, n_rows, nbytes).  Raises UnsupportedTypeException for a schema with a DecimalType field.
+        partition=(row_bytes, var_flags) appends a file's partition values to every row (tfr_batch_rows_with_partition):
+        row_bytes is the UnsafeRow of the partition schema alone, var_flags one 0 / 1 per partition field (1: String,
+        Binary, Decimal with precision > 18)."""
         rp, op = C.c_void_p(), C.c_void_p()
         n, nb = C.c_int64(), C.c_size_t()
-        _check(lib().tfr_batch_rows(self.h, 1 if to_host else 0, C.byref(rp), C.byref(op), C.byref(n), C.byref(nb)))
+        if partition is None:
+            _check(lib().tfr_batch_rows(self.h, 1 if to_host else 0, C.byref(rp), C.byref(op), C.byref(n), C.byref(nb)))
+        else:
+            row, flags = bytes(partition[0]), bytes(bytearray(partition[1]))
+            _check(lib().tfr_batch_rows_with_partition(self.h, 1 if to_host else 0, row, len(row), len(flags), flags,
+                                                       C.byref(rp), C.byref(op), C.byref(n), C.byref(nb)))
         if not to_host:
             return rp.value or 0, op.value or 0, n.value, nb.value
         rows = np.ctypeslib.as_array(C.cast(rp, C.POINTER(C.c_uint8)), shape=(nb.value,)) if nb.value else np.zeros(0, np.uint8)

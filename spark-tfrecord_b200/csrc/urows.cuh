@@ -3,7 +3,8 @@
 // A separate pass over the batch's device columns (the Arrow outputs of any decode path: tile, general, ByteArray, redo);
 // nothing of it runs unless a caller asks for rows.  include/tfrgpu.h restates the layout.  Three steps:
 //   urows_size_kernel : lane = row.  Reads the validity words and the offsets of every column (coalesced at [r]) and sums the
-//                       row's bytes in 64 bits: 8 * (null words + fields), plus each variable value padded to 8 bytes.  It
+//                       row's bytes in 64 bits: 8 * (null words + fields), plus each variable value padded to 8 bytes (and the
+//                       partition row's variable region).  It
 //                       also stores where each variable value starts inside its row (`pos`, [n_var][n_rows]), so that the
 //                       emit kernel can hand fields to its warps independently: recomputing a field's position there would
 //                       cost every warp a walk over all the variable fields in front of it (for string arrays, over their
@@ -15,7 +16,9 @@
 //                       fields w, w + UROWS_WARPS, ...; lane = row writes the null bit and the slot (fixed-width values read at
 //                       [r]), then the value: a short one by its lane, a long one (UROWS_BIG bytes or more) by the whole warp.
 //                       A tile larger than the shared-memory budget is written to global memory by the same code with another
-//                       base pointer.
+//                       base pointer.  Partition values (tfr_batch_rows_with_partition) are the same in every row: the warps
+//                       then share each row's partition null bits, slots and variable region, lane = row, read from a
+//                       small table in global memory that every CTA reads (L1 / L2 hits after the first).
 // Only the batch's column buffers and this pass's own scratch are read.
 //
 // Reference semantics: what Spark's UnsafeProjection makes of the SpecificInternalRow TFRecordDeserializer fills
@@ -43,7 +46,14 @@ struct UrCol {                  // one decoded column (tfr_column), device point
 
 struct UrArgs {
   const UrCol* cols;            // [nf]
-  uint32_t nf, nw, n_rows;
+  uint32_t nf, nw, n_rows;      // nw: null words of the full row, (nf + np + 63) / 64
+  // the partition values (tfr_batch_rows_with_partition), the same in every row: np slots after the nf data slots, null bit
+  // nf + j, and the partition row's variable region (pvw words) at the end of the row.  np = pvw = 0 without them.
+  uint32_t np, pt0, ptn, pvw;   // null words [pt0, pt0 + ptn) hold partition bits
+  const unsigned long long* ptmpl;   // [nw] the partition null bits at their full-row indexes, every other bit zero
+  const unsigned long long* pslot;   // [np] the partition slots; relocated ones hold (offset - Fp) << 32 | size
+  const uint8_t* prel;               // [np] 1: add the row's start of the partition variable region to the offset
+  const unsigned long long* pvar;    // [pvw] the partition row's variable region
   uint32_t* size;               // [n_rows] row bytes (0 for a row that is too large)
   uint32_t* pos;                // [n_var][n_rows] where each variable value starts in its row
   const int64_t* offs;          // [n_rows + 1] row offsets (scan output)
@@ -82,13 +92,14 @@ __device__ __forceinline__ bool ur_present(const UrCol& c, uint32_t r) {
 __global__ void __launch_bounds__(UROWS_SIZE_THREADS) urows_size_kernel(UrArgs A) {
   const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= A.n_rows) return;
-  uint64_t s = 8ull * (A.nw + A.nf);
+  uint64_t s = 8ull * (A.nw + A.nf + A.np);
   for (uint32_t f = 0; f < A.nf; ++f) {
     const UrCol& c = A.cols[f];
     if (c.var < 0) continue;
     A.pos[(size_t)c.var * A.n_rows + r] = (uint32_t)s;
     if (ur_present(c, r)) s += ur_pad8(ur_value_bytes(c, r));
   }
+  s += 8ull * A.pvw;
   const bool big = s > 0x7fffffffull;
   A.size[r] = big ? 0u : (uint32_t)s;
   if (big) atomicMin(A.too_large, r);
@@ -232,6 +243,24 @@ __global__ void __launch_bounds__(UROWS_WARPS * 32) urows_emit_kernel(UrArgs A) 
       mb &= mb - 1;
       uint8_t* d = (uint8_t*)__shfl_sync(FULLMASK, (unsigned long long)(row + p), l);
       ur_emit_warp(c, r0 + (uint32_t)l, d);
+    }
+  }
+  // ---- the partition values: lane = row, warp w takes units w, w + UROWS_WARPS, ... of [the null words holding partition
+  //      bits | the np slots | the variable region's words], so every thread of the CTA shares the constant part ----
+  const uint32_t pn = A.ptn + A.np + A.pvw;
+  if (act && pn) {
+    const uint64_t pv0 = (uint64_t)(A.offs[r + 1] - A.offs[r]) - 8ull * A.pvw;     // where the region starts in this row
+    for (uint32_t k = warp; k < pn; k += UROWS_WARPS) {
+      if (k < A.ptn) {
+        const unsigned long long m = A.ptmpl[A.pt0 + k];
+        if (m) atomicOr(reinterpret_cast<unsigned long long*>(row + 8ull * (A.pt0 + k)), m);   // shares a word with data bits
+      } else if (k < A.ptn + A.np) {
+        const uint32_t j = k - A.ptn;
+        ur_st64(row + 8ull * (A.nw + A.nf + j), A.pslot[j] + (A.prel[j] ? pv0 << 32 : 0ull));
+      } else {
+        const uint32_t i = k - A.ptn - A.np;
+        ur_st64(row + pv0 + 8ull * i, A.pvar[i]);
+      }
     }
   }
   if (!staged) return;

@@ -19,6 +19,8 @@
 //     static native void batchThrowIfError(long batch);   // the exception the reference would throw for the first failing record
 //     static native void batchRelease(long batch);
 //     static native java.nio.ByteBuffer[] batchRows(long batch);   // {rows, int64 row offsets}: pinned UnsafeRows, valid until batchRelease
+//     static native java.nio.ByteBuffer[] batchRowsWithPartition(long batch, java.nio.ByteBuffer partRow, int partRowBytes,
+//                                                                int numPartFields, boolean[] partVar);   // + a file's partition values
 //     static native long encoderCreate(long schema, int device);
 //     static native void encoderDestroy(long encoder);    // OutputWriter.close (M/TFRecordOutputWriter.scala:40-43)
 //     static native java.nio.ByteBuffer encode(long encoder, long[] columnStructAddrs, int n);   // framed bytes, pinned
@@ -166,6 +168,28 @@ extern "C" JNIEXPORT jobjectArray JNICALL Java_com_linkedin_spark_datasources_tf
   const void* rows = nullptr; const int64_t* offs = nullptr; int64_t n = 0; size_t nb = 0;
   int32_t rc = tfr_batch_rows((tfr_batch*)batch, 1, &rows, &offs, &n, &nb);
   if (rc) { throw_for(env, rc, -1); return nullptr; }         // a decimal schema keeps the column views; the batch stays usable
+  jobjectArray out = env->NewObjectArray(2, env->FindClass("java/nio/ByteBuffer"), nullptr);
+  env->SetObjectArrayElement(out, 0, env->NewDirectByteBuffer(const_cast<void*>(rows), (jlong)nb));
+  env->SetObjectArrayElement(out, 1, env->NewDirectByteBuffer(const_cast<int64_t*>(offs), (jlong)((n + 1) * 8)));
+  return out;
+}
+// The same rows with the partition values of the batch's file appended (tfr_batch_rows_with_partition): partRow is a direct
+// buffer holding the UnsafeRow of the partition schema alone (UnsafeProjection.create(partitionSchema)(partitionValues),
+// partRowBytes = its getSizeInBytes), partVar one flag per partition field (String, Binary, Decimal precision > 18).
+extern "C" JNIEXPORT jobjectArray JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_batchRowsWithPartition(
+    JNIEnv* env, jclass, jlong batch, jobject partRow, jint partRowBytes, jint numPartFields, jbooleanArray partVar) {
+  const void* pr = partRow ? env->GetDirectBufferAddress(partRow) : nullptr;
+  std::vector<uint8_t> var;
+  if (partVar) {
+    jboolean* v = env->GetBooleanArrayElements(partVar, nullptr);
+    var.assign(v, v + env->GetArrayLength(partVar));
+    env->ReleaseBooleanArrayElements(partVar, v, JNI_ABORT);
+  }
+  if ((partVar && (jint)var.size() != numPartFields) || partRowBytes < 0) { throw_for(env, TFR_E_INVALID_ARG, -1); return nullptr; }
+  const void* rows = nullptr; const int64_t* offs = nullptr; int64_t n = 0; size_t nb = 0;
+  int32_t rc = tfr_batch_rows_with_partition((tfr_batch*)batch, 1, pr, (size_t)partRowBytes, numPartFields, partVar ? var.data() : nullptr,
+                                             &rows, &offs, &n, &nb);
+  if (rc) { throw_for(env, rc, -1); return nullptr; }
   jobjectArray out = env->NewObjectArray(2, env->FindClass("java/nio/ByteBuffer"), nullptr);
   env->SetObjectArrayElement(out, 0, env->NewDirectByteBuffer(const_cast<void*>(rows), (jlong)nb));
   env->SetObjectArrayElement(out, 1, env->NewDirectByteBuffer(const_cast<int64_t*>(offs), (jlong)((n + 1) * 8)));
