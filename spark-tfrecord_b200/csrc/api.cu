@@ -156,10 +156,16 @@ static int32_t get_ctx(int device, DeviceCtx** out) {
         cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
       }
     }
+    // every handle's kernels read the tables from non-blocking streams, which are not ordered after the legacy default
+    // stream: the copy is complete before any handle of this device exists
     CrcTables* h = new CrcTables;
     build_crc_tables(*h);
-    c.err = cudaMalloc(&c.d_tabs, sizeof(CrcTables));
-    if (c.err == cudaSuccess) c.err = cudaMemcpy(c.d_tabs, h, sizeof(CrcTables), cudaMemcpyHostToDevice);
+    cudaStream_t st = nullptr;
+    c.err = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
+    if (c.err == cudaSuccess) c.err = cudaMalloc(&c.d_tabs, sizeof(CrcTables));
+    if (c.err == cudaSuccess) c.err = cudaMemcpyAsync(c.d_tabs, h, sizeof(CrcTables), cudaMemcpyHostToDevice, st);
+    if (c.err == cudaSuccess) c.err = cudaStreamSynchronize(st);
+    if (st) cudaStreamDestroy(st);
     delete h;
   });
   if (c.err != cudaSuccess) return fail(TFR_E_CUDA, std::string("device init: ") + cudaGetErrorString(c.err));
@@ -253,22 +259,23 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
 extern "C" void tfr_schema_destroy(tfr_schema* s) { delete s; }
 extern "C" int32_t tfr_schema_num_fields(const tfr_schema* s) { return s ? (int32_t)s->fields.size() : 0; }
 
-// device copy of a schema
+// device copy of a schema.  The copies run on the handle's stream `st` and are waited for before returning: the handle's
+// kernels run on non-blocking streams, which nothing orders after the legacy default stream, and `tp` is a local.
 struct DevSchemaBuf {
   DevField* d_fields = nullptr; uint8_t* d_names = nullptr; int32_t* d_ht = nullptr; int32_t* d_var_field = nullptr;
   FieldTemplate* d_templates = nullptr;
   uint8_t* d_tile_consts = nullptr; uint32_t tile_consts_bytes = 0;     // tile.cuh: per-schema constants in the shared-memory layout
   DevSchema view{};
-  int32_t upload(const tfr_schema& s) {
+  int32_t upload(const tfr_schema& s, cudaStream_t st) {
     size_t nf = s.fields.size();
     CUDA_TRY(cudaMalloc(&d_fields, std::max<size_t>(1, nf) * sizeof(DevField)));
     CUDA_TRY(cudaMalloc(&d_names, std::max<size_t>(1, s.names.size())));
     CUDA_TRY(cudaMalloc(&d_ht, s.ht.size() * sizeof(int32_t)));
     CUDA_TRY(cudaMalloc(&d_var_field, std::max<size_t>(1, s.var_field.size()) * sizeof(int32_t)));
-    if (nf) CUDA_TRY(cudaMemcpy(d_fields, s.fields.data(), nf * sizeof(DevField), cudaMemcpyHostToDevice));
-    if (!s.names.empty()) CUDA_TRY(cudaMemcpy(d_names, s.names.data(), s.names.size(), cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(d_ht, s.ht.data(), s.ht.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-    if (!s.var_field.empty()) CUDA_TRY(cudaMemcpy(d_var_field, s.var_field.data(), s.var_field.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+    if (nf) CUDA_TRY(cudaMemcpyAsync(d_fields, s.fields.data(), nf * sizeof(DevField), cudaMemcpyHostToDevice, st));
+    if (!s.names.empty()) CUDA_TRY(cudaMemcpyAsync(d_names, s.names.data(), s.names.size(), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_ht, s.ht.data(), s.ht.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    if (!s.var_field.empty()) CUDA_TRY(cudaMemcpyAsync(d_var_field, s.var_field.data(), s.var_field.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     {
       // canonical entry prefix of every field: 0A ? 0A klen key 12 ? kindtag ?   (? = length bytes, masked out)
       std::vector<FieldTemplate> tp(std::max<size_t>(1, nf));
@@ -289,7 +296,8 @@ struct DevSchemaBuf {
         memcpy(t.words, bytes, sizeof bytes); memcpy(t.mask, mask, sizeof mask);
       }
       CUDA_TRY(cudaMalloc(&d_templates, tp.size() * sizeof(FieldTemplate)));
-      CUDA_TRY(cudaMemcpy(d_templates, tp.data(), tp.size() * sizeof(FieldTemplate), cudaMemcpyHostToDevice));
+      CUDA_TRY(cudaMemcpyAsync(d_templates, tp.data(), tp.size() * sizeof(FieldTemplate), cudaMemcpyHostToDevice, st));
+      CUDA_TRY(cudaStreamSynchronize(st));
     }
     view.n_fields = (int32_t)nf; view.record_type = s.record_type; view.ht_mask = (int32_t)s.ht.size() - 1;
     view.n_fix = s.n_fix; view.n_var = s.n_var; view.n_cnt = s.n_cnt;
@@ -297,32 +305,40 @@ struct DevSchemaBuf {
     return TFR_OK;
   }
   // CRC tables | zeroed seen words | DevField[nf] | FieldTemplate[nf] | names, each section 16-byte aligned (tile_const_bytes)
-  int32_t build_tile_consts(const tfr_schema& s, const CrcTables* d_tabs) {
+  int32_t build_tile_consts(const tfr_schema& s, const CrcTables* d_tabs, cudaStream_t st) {
     const uint32_t nf = (uint32_t)s.fields.size(), nb = (uint32_t)s.names.size();
     tile_consts_bytes = tile_const_bytes(nf, nb);
     CUDA_TRY(cudaMalloc(&d_tile_consts, tile_consts_bytes));
-    CUDA_TRY(cudaMemset(d_tile_consts, 0, tile_consts_bytes));
+    CUDA_TRY(cudaMemsetAsync(d_tile_consts, 0, tile_consts_bytes, st));
     uint8_t* q = d_tile_consts;
-    CUDA_TRY(cudaMemcpy(q, d_tabs->g5, TILE_CRC_BYTES, cudaMemcpyDeviceToDevice));   // g5 then xp16, contiguous in CrcTables
+    CUDA_TRY(cudaMemcpyAsync(q, d_tabs->g5, TILE_CRC_BYTES, cudaMemcpyDeviceToDevice, st));   // g5 then xp16, contiguous in CrcTables
     q += TILE_CRC_BYTES + TILE_SEEN_BYTES;
-    if (nf) CUDA_TRY(cudaMemcpy(q, d_fields, nf * sizeof(DevField), cudaMemcpyDeviceToDevice));
+    if (nf) CUDA_TRY(cudaMemcpyAsync(q, d_fields, nf * sizeof(DevField), cudaMemcpyDeviceToDevice, st));
     q += (nf * sizeof(DevField) + 15) & ~(size_t)15;
-    if (nf) CUDA_TRY(cudaMemcpy(q, d_templates, nf * sizeof(FieldTemplate), cudaMemcpyDeviceToDevice));
+    if (nf) CUDA_TRY(cudaMemcpyAsync(q, d_templates, nf * sizeof(FieldTemplate), cudaMemcpyDeviceToDevice, st));
     q += (nf * sizeof(FieldTemplate) + 15) & ~(size_t)15;
-    if (nb) CUDA_TRY(cudaMemcpy(q, d_names, nb, cudaMemcpyDeviceToDevice));
+    if (nb) CUDA_TRY(cudaMemcpyAsync(q, d_names, nb, cudaMemcpyDeviceToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));             // the decoder's kernels read these from its other streams too
     return TFR_OK;
   }
   void free_all() { cudaFree(d_fields); cudaFree(d_names); cudaFree(d_ht); cudaFree(d_var_field); cudaFree(d_templates); cudaFree(d_tile_consts); }
 };
 
-// Raises Kernel's opt-in dynamic shared memory to `smem` bytes on the current device, once per device and size
+// Raises Kernel's opt-in dynamic shared memory to at least `smem` bytes on the current device; never lowers it.
+// cudaFuncSetAttribute sets the limit, it does not take a maximum, and every thread of the process launches the same kernels:
+// the check and the set happen under one lock, so that a thread asking for less cannot overwrite a larger grant another thread
+// has just made (which would leave `granted` above the attribute and fail every later launch between the two sizes).
+// `granted` only changes after the attribute does, so a value read without the lock that is already large enough is safe.
+static std::mutex g_dyn_smem_mu;
 template <auto Kernel>
 static cudaError_t raise_dyn_smem(size_t smem) {
-  static size_t granted[64] = {0};                      // per device
+  static std::atomic<size_t> granted[64];               // per device; zero-initialised (static storage)
   int dev = 0; cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64 || granted[dev] >= smem) return cudaSuccess;
+  if (dev < 0 || dev >= 64 || granted[dev].load(std::memory_order_acquire) >= smem) return cudaSuccess;
+  std::lock_guard<std::mutex> lk(g_dyn_smem_mu);
+  if (granted[dev].load(std::memory_order_relaxed) >= smem) return cudaSuccess;
   cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e == cudaSuccess) granted[dev] = smem;
+  if (e == cudaSuccess) granted[dev].store(smem, std::memory_order_release);
   return e;
 }
 
