@@ -349,6 +349,55 @@ int32_t tfr_encode_rows(tfr_encoder*, const void* rows, const int32_t* row_offse
 int32_t tfr_encoder_result_host(tfr_encoder*, void** host_ptr, size_t* nbytes);
 int32_t tfr_encoder_stream(tfr_encoder*, void** cuda_stream);
 
+/* ---- pipelined encode of UnsafeRow batches ---------------------------------------------
+ * tfr_encode_rows_submit is the pipelined form of tfr_encode_rows: it enqueues the copy of the rows, the row kernels, the
+ * encode and the copy of the framed bytes to pinned host memory, and returns without waiting, so that a writer task can
+ * fill the next batch of rows while the GPU encodes this one.  The H2D of batch k+1, the kernels of batch k and the D2H of
+ * batch k-1 run at the same time.  Each submission owns its result; a tfr_encoded handle is thread-confined like its encoder.
+ *   Input        : the layout and the semantics of tfr_encode_rows, for Example, SequenceExample and ByteArray schemas.
+ *                  Host input must stay unchanged until the submission has been waited on or released; device input
+ *                  until it has been waited on (a batch the pipelined kernels could not vouch for is encoded again from it).
+ *   Staging      : tfr_encoder_num_row_slots() pinned buffers; slot 0 is the buffer tfr_encoder_row_staging returns.
+ *                  Rows staged in slot k go through pipeline lane k.  A slot may be refilled once the submission that read
+ *                  it has been waited on or released.
+ *   Synchronisation : once the encoder has learned its sizes, submitting rows that sit in slot staging does no host
+ *                  synchronisation.  Device input keeps the one read-back of row_offsets[0] and row_offsets[n_rows] that
+ *                  tfr_encode_rows does.
+ *   Learning     : the first submission of an encoder runs the synchronous path before it returns.  Later ones are sized
+ *                  from the last clean batch (framed bytes per input byte, largest record, longest ByteArray payload);
+ *                  the device checks those figures, and tfr_encoded_wait redoes -- transparently, with identical results --
+ *                  any batch they did not fit.  A redo teaches the encoder its sizes, so the submission after it is pipelined
+ *                  again.  A data error (a null or a malformed row) leaves what was learned as it was.
+ *   Depth        : at most tfr_encoder_num_row_slots() submissions are in flight; a further submit first waits for the
+ *                  oldest one on its lane.
+ *   Errors       : tfr_encode_rows_submit returns only argument errors (those of tfr_encode_rows: null pointers, misaligned
+ *                  rows, n_rows >= 2^31 as TFR_E_BATCH_TOO_LARGE), TFR_E_OOM and TFR_E_CUDA.  tfr_encoded_wait returns
+ *                  exactly the status, *error_row and tfr_last_error class tfr_encode_rows returns for the same rows (a
+ *                  malformed row wins over a null at the same or a later row; TFR_E_BATCH_TOO_LARGE).  A failed
+ *                  submission has no bytes.
+ *   Results      : tfr_encoded_result: to_host = 0 the device bytes, 1 the pinned host bytes; byte-identical to
+ *                  tfr_encode_rows followed by tfr_encoder_result_host.  Valid until tfr_encoded_release; the call waits
+ *                  first if needed.
+ *   Release      : without a wait is allowed; the submission's buffers go back to its lane when its work has run, with no
+ *                  host wait.  tfr_encoded_release(NULL) does nothing.
+ *   Mixing calls : tfr_encode, tfr_encode_rows, and a staging call that grows a slot, first wait for the submissions in
+ *                  flight; their results stay valid.  tfr_encoder_result_host keeps returning the last synchronous call's
+ *                  result.
+ *   Destroy      : tfr_encoder_destroy waits for and frees everything, unreleased submissions included; using such a
+ *                  handle afterwards is a caller error.
+ * tfr_encoder_get_stats: counters since creation: [0] submissions, [1] enqueued without a host synchronisation, [2] of those
+ * redone after the device raised a flag, [3] results whose host copy needed a top-up at wait (the batch was larger than
+ * predicted, within the head-room), [4] submissions that ran the general (non-tile) emit kernel.                        */
+typedef struct tfr_encoded tfr_encoded;
+int32_t tfr_encoder_num_row_slots(void);
+int32_t tfr_encoder_row_staging_slot(tfr_encoder*, int32_t slot, size_t min_bytes, void** host_ptr, size_t* capacity);
+int32_t tfr_encode_rows_submit(tfr_encoder*, const void* rows, const int32_t* row_offsets, int64_t n_rows,
+                               int32_t on_device, tfr_encoded** out);
+int32_t tfr_encoded_wait(tfr_encoded*, int64_t* error_row);
+int32_t tfr_encoded_result(tfr_encoded*, int32_t to_host, void** ptr, size_t* nbytes);
+void    tfr_encoded_release(tfr_encoded*);
+int32_t tfr_encoder_get_stats(tfr_encoder*, int64_t* out, int32_t n /* <= 8 */);
+
 /* ---- schema inference (SURVEY.md 8f.1; M/TensorFlowInferSchema.scala:35-58) ------------ */
 /* lattice codes of M/TensorFlowInferSchema.scala:194-207; merge = max, 0 = identity     */
 enum { TFR_INF_NULL = 0, TFR_INF_LONG = 1, TFR_INF_FLOAT = 2, TFR_INF_STRING = 3,

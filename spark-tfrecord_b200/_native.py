@@ -27,7 +27,8 @@ EXPORTS = [
     "tfr_batch_to_host_async", "tfr_batch_to_host", "tfr_batch_export_arrow_host", "tfr_batch_export_arrow_device", "tfr_batch_release",
     "tfr_batch_rows", "tfr_batch_rows_with_partition",
     "tfr_encoder_create", "tfr_encoder_destroy", "tfr_encode", "tfr_encoder_row_staging", "tfr_encode_rows", "tfr_encoder_result_host",
-    "tfr_encoder_stream",
+    "tfr_encoder_stream", "tfr_encoder_num_row_slots", "tfr_encoder_row_staging_slot", "tfr_encode_rows_submit", "tfr_encoded_wait",
+    "tfr_encoded_result", "tfr_encoded_release", "tfr_encoder_get_stats",
     "tfr_infer_create", "tfr_infer_update", "tfr_infer_update_block", "tfr_infer_result", "tfr_infer_name", "tfr_infer_destroy",
 ]
 
@@ -134,6 +135,13 @@ def lib():
         "tfr_encode_rows": (i32, [vp, vp, vp, i64, i32, P(vp), P(sz), P(i64)]),
         "tfr_encoder_result_host": (i32, [vp, P(vp), P(sz)]),
         "tfr_encoder_stream": (i32, [vp, P(vp)]),
+        "tfr_encoder_num_row_slots": (i32, []),
+        "tfr_encoder_row_staging_slot": (i32, [vp, i32, sz, P(vp), P(sz)]),
+        "tfr_encode_rows_submit": (i32, [vp, vp, vp, i64, i32, P(vp)]),
+        "tfr_encoded_wait": (i32, [vp, P(i64)]),
+        "tfr_encoded_result": (i32, [vp, i32, P(vp), P(sz)]),
+        "tfr_encoded_release": (None, [vp]),
+        "tfr_encoder_get_stats": (i32, [vp, P(i64), i32]),
         "tfr_infer_create": (i32, [i32, i32, P(vp)]),
         "tfr_infer_update": (i32, [vp, vp, sz, i32]),
         "tfr_infer_result": (i32, [vp, P(i32)]),
@@ -435,6 +443,43 @@ class Encoder:
         _check(lib().tfr_encoder_result_host(self.h, C.byref(p), C.byref(nb)))
         return C.string_at(p, nb.value)
 
+    @staticmethod
+    def num_row_slots() -> int:
+        return lib().tfr_encoder_num_row_slots()
+
+    def row_staging_slot(self, slot: int, nbytes: int) -> np.ndarray:
+        """pinned row staging of pipeline slot `slot` (slot 0 is row_staging); refill it once the submission that read it
+        has been waited on or released"""
+        p = C.c_void_p()
+        cap = C.c_size_t()
+        _check(lib().tfr_encoder_row_staging_slot(self.h, slot, nbytes, C.byref(p), C.byref(cap)))
+        return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=(cap.value,))
+
+    def submit_rows(self, rows, offsets, on_device: Optional[bool] = None) -> "Encoded":
+        """pipelined encode_rows (tfr_encode_rows_submit): returns at once; Encoded.wait() raises what encode_rows raises"""
+        rp, _, rdev, keep_r = _device_ptr(rows)
+        if not isinstance(offsets, tuple):
+            try:
+                import torch
+                is_t = isinstance(offsets, torch.Tensor)
+            except ImportError:
+                is_t = False
+            offsets = offsets.to(torch.int32) if is_t else np.asarray(offsets, dtype=np.int32)
+        op, onb, odev, keep_o = _device_ptr(offsets)
+        if rdev != odev:
+            raise ValueError("rows and offsets must both be host or both be device memory")
+        n_rows = onb // 4 - 1 if not isinstance(offsets, tuple) else offsets[1] // 4 - 1
+        dev = rdev if on_device is None else (1 if on_device else 0)
+        h = C.c_void_p()
+        _check(lib().tfr_encode_rows_submit(self.h, rp, op, max(n_rows, 0), dev, C.byref(h)))
+        return Encoded(h, self, (keep_r, keep_o))
+
+    def stats(self) -> dict:
+        v = (C.c_int64 * 8)()
+        _check(lib().tfr_encoder_get_stats(self.h, v, 8))
+        names = ["submits", "speculative_submits", "speculative_redone", "host_topups", "general_emit"]
+        return {k: v[i] for i, k in enumerate(names)}
+
     def stream(self) -> int:
         p = C.c_void_p()
         _check(lib().tfr_encoder_stream(self.h, C.byref(p)))
@@ -449,6 +494,51 @@ class Encoder:
     def __del__(self):
         try:
             self.close()
+        except Exception:
+            pass
+
+
+class Encoded:
+    """One pipelined encode (Encoder.submit_rows).  Every accessor waits for it first; the bytes stay valid until release()."""
+
+    def __init__(self, h, enc, keep=None):
+        self.h = h
+        self.enc = enc
+        self._keep = keep          # the input of a pending submission must outlive it
+
+    def wait(self):
+        """raises the TfrError subclass (with .row) encode_rows raises for the same rows"""
+        er = C.c_int64(-1)
+        rc = lib().tfr_encoded_wait(self.h, C.byref(er))
+        if rc != 0:
+            msg = lib().tfr_last_error()
+            raise error_for(rc, msg.decode("utf-8", "replace") if msg else "", er.value)
+
+    def _result(self, to_host: int):
+        self.wait()
+        p = C.c_void_p()
+        nb = C.c_size_t()
+        _check(lib().tfr_encoded_result(self.h, to_host, C.byref(p), C.byref(nb)))
+        return p.value or 0, nb.value
+
+    def result_host(self) -> bytes:
+        p, n = self._result(1)
+        return C.string_at(p, n) if n else b""
+
+    def result_device(self):
+        """-> (device ptr, nbytes)"""
+        return self._result(0)
+
+    def release(self):
+        # after Encoder.close() the encoder has freed every submission already
+        if self.h and self.enc.h:
+            lib().tfr_encoded_release(self.h)
+        self.h = None
+        self._keep = None
+
+    def __del__(self):
+        try:
+            self.release()
         except Exception:
             pass
 

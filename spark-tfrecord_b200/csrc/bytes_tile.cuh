@@ -193,8 +193,12 @@ __global__ void bytes_max_len_kernel(const int32_t* __restrict__ offs, uint32_t 
   if ((threadIdx.x & 31) == 0 && m) atomicMax(out, m);
 }
 
-template <int CW, int XW>
-__global__ void BYTES_BOUNDS(CW, XW) encode_bytes_kernel(EncBytesArgs A) {
+// GUARD: the pipelined encoder's instantiation (api_encode.inc): it returns at once when encode_verdict_kernel (encode.cuh) has
+// raised *flag -- the stride was launched for a learned payload length the batch exceeds, the output block is too small, or the
+// batch holds a data error.  GUARD = false (the synchronous path) never reads `flag`.
+template <int CW, int XW, bool GUARD>
+__global__ void BYTES_BOUNDS(CW, XW) encode_bytes_kernel(EncBytesArgs A, const uint32_t* __restrict__ flag) {
+  if (GUARD && *flag) return;
   extern __shared__ __align__(128) uint8_t smem_raw[];
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw);
   uint32_t* s8 = reinterpret_cast<uint32_t*>(smem_raw + 16);

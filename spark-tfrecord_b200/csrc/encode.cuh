@@ -150,8 +150,11 @@ __device__ __forceinline__ uint32_t warp_excl_scan(uint32_t v, uint32_t& total) 
 }
 
 // mode 0: sizes; mode 1: emit
-template <int MODE>
-__global__ void __launch_bounds__(256) encode_kernel(EncodeArgs A) {
+// GUARD (MODE 1 only): the pipelined encoder's emit (api_encode.inc), which returns at once when encode_verdict_kernel (below)
+// has raised *flag.  GUARD = false never reads `flag`.
+template <int MODE, bool GUARD>
+__global__ void __launch_bounds__(256) encode_kernel(EncodeArgs A, const uint32_t* __restrict__ flag) {
+  if (GUARD && *flag) return;
   extern __shared__ uint32_t smem[];
   uint32_t* stab = smem;
   if (MODE == 1) { crc_stage_tables(stab, A.tabs); __syncthreads(); }
@@ -254,4 +257,42 @@ __global__ void __launch_bounds__(256) encode_kernel(EncodeArgs A) {
       for (int i = 0; i < 4; ++i) { rec[8 + i] = (uint8_t)(hc >> (8 * i)); rec[12 + plen + i] = (uint8_t)(crc >> (8 * i)); }
     }
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Verdict of a pipelined encode (api_encode.inc, tfr_encode_rows_submit).  Its outputs were sized from what the encoder
+// learned on earlier batches, not from this batch's sizes; one thread checks them after the record-size scan and raises
+// v[EV_FLAG] when the batch cannot be emitted as launched.  The guarded emit kernels read that word first, so a flagged batch
+// writes nothing; the host redoes it through the synchronous path.  The total and the first error rows go to the verdict too.
+// ---------------------------------------------------------------------------------------------
+enum { EV_FLAG = 16, EV_TOTAL_LO = 17, EV_TOTAL_HI = 18 };     // words of the encoder's small block, behind the ones of encode.cuh / rows.cuh
+enum { EVF_CAPACITY = 1, EVF_SLOT = 2, EVF_STRIDE = 4, EVF_ROWS = 8, EVF_NULL = 16 };
+struct EncVerdictArgs {
+  uint32_t* small;                       // [0] first null row, [1] scan overflow, [4] largest framed record / payload, [8..10] row path
+  const unsigned long long* total;       // Example / SequenceExample: the scan's grand total
+  const int32_t* bytes_offs;             // ByteArray: the column's offsets (total = offs[n] - offs[0] + 16 n); null otherwise
+  uint32_t n_rows;
+  unsigned long long cap;                // bytes of the output block
+  uint32_t max_rec;                      // largest framed record the tile slot holds (0: the general emit kernel, no limit)
+  uint32_t max_len;                      // ByteArray: largest payload the launched stride holds
+};
+__global__ void encode_verdict_kernel(EncVerdictArgs A) {
+  if (threadIdx.x | blockIdx.x) return;
+  uint32_t* s = A.small;
+  uint32_t flag = 0;
+  unsigned long long total;
+  if (A.bytes_offs) {
+    const int32_t o0 = A.bytes_offs[0], on = A.bytes_offs[A.n_rows];
+    total = on >= o0 && o0 >= 0 ? (unsigned long long)(on - o0) + 16ull * A.n_rows : ~0ull;
+    if (s[4] > A.max_len) flag |= EVF_STRIDE;
+  } else {
+    total = *A.total;
+    if (s[1]) flag |= EVF_CAPACITY;
+    if (A.max_rec && s[4] > A.max_rec) flag |= EVF_SLOT;
+  }
+  if (total > A.cap || total > 0x7fffffffull) flag |= EVF_CAPACITY;
+  if (s[8] != 0xffffffffu || s[9] != 0xffffffffu || s[10]) flag |= EVF_ROWS;
+  if (s[0] != 0xffffffffu) flag |= EVF_NULL;
+  s[EV_FLAG] = flag;
+  s[EV_TOTAL_LO] = (uint32_t)total; s[EV_TOTAL_HI] = (uint32_t)(total >> 32);
 }

@@ -102,7 +102,12 @@ __global__ void __launch_bounds__(ENC_SIZE_THREADS, 6) encode_tile_size_kernel(E
   }
 }
 
-__global__ void __launch_bounds__(ENC_TILE_THREADS, 3) encode_tile_kernel(EncTileArgs A) {
+// GUARD: the instantiation of the pipelined encoder (api_encode.inc).  Its launch figures were learned on earlier batches, so it
+// returns at once when encode_verdict_kernel (encode.cuh) has raised *flag: the output block or the slot would be too small, or
+// the batch holds a data error.  GUARD = false (the synchronous path) never reads `flag`.
+template <bool GUARD>
+__global__ void __launch_bounds__(ENC_TILE_THREADS, 3) encode_tile_kernel(EncTileArgs A, const uint32_t* __restrict__ flag) {
+  if (GUARD && *flag) return;
   extern __shared__ __align__(128) uint8_t esm[];
   uint32_t* g5 = reinterpret_cast<uint32_t*>(esm);
   const uint32_t* xp16 = g5 + 512;

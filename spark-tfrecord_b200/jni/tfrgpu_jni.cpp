@@ -26,6 +26,11 @@
 //     static native java.nio.ByteBuffer encode(long encoder, long[] columnStructAddrs, int n);   // framed bytes, pinned
 //     static native java.nio.ByteBuffer encoderRowStaging(long encoder, long minBytes);          // direct, pinned: UnsafeRow bytes
 //     static native java.nio.ByteBuffer encodeRows(long encoder, java.nio.ByteBuffer rows, java.nio.ByteBuffer offsets, int nRows);
+//     static native int encoderRowSlots();                                                        // pipelined RowWriter (INTEGRATION.md)
+//     static native java.nio.ByteBuffer encoderRowStagingSlot(long encoder, int slot, long minBytes);   // direct, pinned: slot k's rows
+//     static native long encodeRowsSubmit(long encoder, java.nio.ByteBuffer rows, java.nio.ByteBuffer offsets, int nRows);   // -> handle
+//     static native java.nio.ByteBuffer encodedWait(long encoded);   // framed bytes, pinned, valid until encodedRelease
+//     static native void encodedRelease(long encoded);
 //     static native long inferCreate(int recordType, int device);                                 // DefaultSource.inferSchema (M/DefaultSource.scala:31-39)
 //     static native long inferUpdate(long infer, java.nio.ByteBuffer block, long nbytes, boolean isFinal);   // -> consumed bytes
 //     static native Object[] inferResult(long infer);     // {String[] names (bytewise sorted), int[] lattice codes}
@@ -241,6 +246,47 @@ extern "C" JNIEXPORT jobject JNICALL Java_com_linkedin_spark_datasources_tfrecor
   rc = tfr_encoder_result_host((tfr_encoder*)enc, &host, &nb);
   if (rc) { throw_for(env, rc, -1); return nullptr; }
   return env->NewDirectByteBuffer(host, (jlong)nb);
+}
+
+// ---- pipelined row path (INTEGRATION.md, RowWriter): flush k is submitted from slot k and waited for before the slot is refilled ----
+static void throw_for_rows(JNIEnv* env, int32_t rc, int64_t err_row) {
+  if (rc == TFR_E_INVALID_ARG) {
+    std::string msg = "malformed UnsafeRow" + (err_row >= 0 ? " (row " + std::to_string(err_row) + ")" : std::string()) + ": " + tfr_last_error();
+    env->ThrowNew(env->FindClass("java/lang/IllegalArgumentException"), msg.c_str());
+    return;
+  }
+  throw_for(env, rc, err_row);
+}
+extern "C" JNIEXPORT jint JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_encoderRowSlots(JNIEnv*, jclass) { return tfr_encoder_num_row_slots(); }
+extern "C" JNIEXPORT jobject JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_encoderRowStagingSlot(JNIEnv* env, jclass, jlong enc, jint slot,
+                                                                                                            jlong minBytes) {
+  void* p = nullptr; size_t cap = 0;
+  int32_t rc = tfr_encoder_row_staging_slot((tfr_encoder*)enc, (int32_t)slot, (size_t)minBytes, &p, &cap);
+  if (rc) { throw_for(env, rc, -1); return nullptr; }
+  return env->NewDirectByteBuffer(p, (jlong)cap);
+}
+// returns at once; the rows and offsets buffers must stay unchanged until encodedWait (or encodedRelease)
+extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_encodeRowsSubmit(JNIEnv* env, jclass, jlong enc, jobject rows,
+                                                                                                     jobject offsets, jint nRows) {
+  tfr_encoded* h = nullptr;
+  int32_t rc = tfr_encode_rows_submit((tfr_encoder*)enc, env->GetDirectBufferAddress(rows), (const int32_t*)env->GetDirectBufferAddress(offsets),
+                                      (int64_t)nRows, 0, &h);
+  if (rc) { throw_for_rows(env, rc, -1); return 0; }
+  return (jlong)h;
+}
+// the framed bytes of the flush (what encodeRows returns for the same rows), or the exception encodeRows throws, with its row;
+// a failed flush is released before the exception is thrown
+extern "C" JNIEXPORT jobject JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_encodedWait(JNIEnv* env, jclass, jlong encoded) {
+  tfr_encoded* h = (tfr_encoded*)encoded;
+  int64_t err_row = -1;
+  int32_t rc = tfr_encoded_wait(h, &err_row);
+  void* host = nullptr; size_t nb = 0;
+  if (!rc) rc = tfr_encoded_result(h, 1, &host, &nb);
+  if (rc) { tfr_encoded_release(h); throw_for_rows(env, rc, err_row); return nullptr; }
+  return env->NewDirectByteBuffer(host, (jlong)nb);
+}
+extern "C" JNIEXPORT void JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_encodedRelease(JNIEnv*, jclass, jlong encoded) {
+  if (encoded) tfr_encoded_release((tfr_encoded*)encoded);
 }
 
 // ---- schema inference: DefaultSource.inferSchema -> TensorFlowInferSchema (M/DefaultSource.scala:31-39,48-70) ----
