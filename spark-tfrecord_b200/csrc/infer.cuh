@@ -7,13 +7,17 @@
 // ArrayType(ArrayType(T)) (7..9) :98-118); codes of one name merge with findTightestCommonType = max with
 // null as identity (:213-228).  Here: warp per record, one map entry per lane (the full-semantics parser of
 // decode.cuh), duplicate keys inside a record resolved last-wins before anything is merged, then one
-// atomicMax per (name, record) into a device hash table keyed by a 64-bit hash of the name.
+// atomicMax per (name, record) into a device hash table.  A 64-bit hash of the name picks the slot and filters,
+// names are equal only when their bytes are.
+// A record's verdict is the reference's: a CRC or parse failure anywhere in the record (parseFrom throws before
+// inference sees a value), else the first value error of the surviving entries in map order (the position of a key's
+// first occurrence), context before feature_lists.
 #pragma once
 #include "common.cuh"
 #include "decode.cuh"
 
 struct InferSlot {
-  unsigned long long hash;   // 0 = empty
+  unsigned long long hash;   // 0 = empty, INFER_CLAIMED = name being written
   uint32_t name_off;         // offset of the key bytes inside the batch that first inserted the name
   uint32_t name_len;
   uint32_t code;             // max lattice code seen (0..9)
@@ -21,7 +25,10 @@ struct InferSlot {
 };
 #define INFER_TABLE_SLOTS 65536u
 #define INFER_MAX_ENT 1024     // entries of one map buffered per record for last-wins de-duplication; more raise INF_OVF_ENTRIES
+#define INFER_CLAIMED (~0ull)  // a slot whose name is being written: its hash is published after the name
 enum { INF_OVF_TABLE = 1u, INF_OVF_ENTRIES = 2u, INF_OVF_KEY = 4u };   // limits hit: reported as an explicit error, never as a silently wrong schema
+// per-entry record in shared memory: ecode = lattice code (bits 0-3) | value error (bits 4-7, INF_ERR_*) | key length << 8
+enum { INF_ERR_KIND = 1u, INF_ERR_EMPTY = 2u };
 
 struct InferArgs {
   const uint8_t* data;
@@ -31,14 +38,19 @@ struct InferArgs {
   uint32_t record_type;
   const CrcTables* tabs;
   InferSlot* table;
-  uint32_t* first_err;       // [0] min failing record index, [1] INF_OVF_* flags
+  uint32_t* first_err;       // [0] min failing record index, [1] INF_OVF_* flags, [4] min record index over a per-record limit
   uint32_t* status;          // [n]
 };
 
 __device__ __forceinline__ unsigned long long hash64(const uint8_t* p, uint32_t n) {
   unsigned long long h = 1469598103934665603ull;
   for (uint32_t i = 0; i < n; ++i) h = (h ^ p[i]) * 1099511628211ull;
-  return h ? h : 1ull;
+  return (h == 0ull || h == INFER_CLAIMED) ? 1ull : h;          // 0 and INFER_CLAIMED mark slots
+}
+__device__ __forceinline__ bool bytes_equal(const uint8_t* a, const uint8_t* b, uint32_t n) {
+  if (a == b) return true;
+  for (uint32_t i = 0; i < n; ++i) if (a[i] != b[i]) return false;
+  return true;
 }
 __device__ __forceinline__ int feat_code(const FeatAcc& a) {       // inferField + parse*List
   if (a.kind == K_NONE) return -1;                                  // RuntimeException("unsupported type ...")
@@ -46,36 +58,56 @@ __device__ __forceinline__ int feat_code(const FeatAcc& a) {       // inferField
   int base = a.kind == K_INT64 ? 1 : a.kind == K_FLOAT ? 2 : 3;
   return a.n > 1 ? base + 3 : base;
 }
-__device__ __forceinline__ void infer_merge(InferSlot* table, unsigned long long h, uint32_t name_off, uint32_t name_len, int code, uint32_t* ovf) {
+// Names are substrings of the block being inferred (A.data): the table is cleared before and gathered after every block.
+__device__ __forceinline__ void infer_merge(InferSlot* table, const uint8_t* data, unsigned long long h, uint32_t name_off, uint32_t name_len,
+                                            int code, uint32_t* ovf) {
   uint32_t slot = (uint32_t)(h ^ (h >> 32)) & (INFER_TABLE_SLOTS - 1);
   for (uint32_t probe = 0; probe < INFER_TABLE_SLOTS; ++probe) {
-    unsigned long long cur = atomicCAS(&table[slot].hash, 0ull, h);
-    if (cur == 0ull) { table[slot].name_off = name_off; table[slot].name_len = name_len; cur = h; }
-    if (cur == h) {
-      if (code == 10) atomicOr(&table[slot].flags, 1u);
-      else atomicMax(&table[slot].code, (uint32_t)code);
+    InferSlot* s = &table[slot];
+    unsigned long long cur = atomicCAS(&s->hash, 0ull, INFER_CLAIMED);
+    bool same = false;
+    if (cur == 0ull) {
+      // claimed: write the name, then publish the hash; a reader that sees the hash sees the name
+      s->name_off = name_off; s->name_len = name_len;
+      __threadfence();
+      atomicExch(&s->hash, h);
+      same = true;
+    } else {
+      // another thread (maybe a lane of this warp) is writing this slot's name: independent thread scheduling lets it finish
+      while (cur == INFER_CLAIMED) { __nanosleep(20); cur = *(volatile unsigned long long*)&s->hash; }
+      if (cur == h) {
+        __threadfence();
+        const uint32_t off = *(volatile uint32_t*)&s->name_off, len = *(volatile uint32_t*)&s->name_len;
+        same = len == name_len && bytes_equal(data + off, data + name_off, len);
+      }
+    }
+    if (same) {
+      if (code == 10) atomicOr(&s->flags, 1u);
+      else atomicMax(&s->code, (uint32_t)code);
       return;
     }
-    slot = (slot + 1) & (INFER_TABLE_SLOTS - 1);
+    slot = (slot + 1) & (INFER_TABLE_SLOTS - 1);            // empty-to-us, another hash, or the same hash and other bytes
   }
   atomicOr(ovf, INF_OVF_TABLE);            // more distinct names than slots
 }
 
-// one map (Features or FeatureLists) of one record: entries -> (hash, code, key) in shared memory, last wins, merge
+// one map (Features or FeatureLists) of one record: entries -> (hash, code | value error, key) in shared memory.  Returns
+// false when the map does not parse; `over` is set when the map passes a per-record limit (entries, key length).
 __device__ __forceinline__ bool infer_map(const InferArgs& A, Cur body, bool is_flist, unsigned long long* eh, uint32_t* ecode, uint32_t* ekey,
-                                          uint32_t& nent, int& err) {
+                                          uint32_t& nent, bool& over) {
   const uint32_t lane = threadIdx.x & 31;
   // (1) uniform hop collecting entry ranges; 32 at a time parsed one per lane
   uint32_t pend = 0, my_len = 0;
   const uint8_t* my_ptr = nullptr;
   auto flush = [&]() -> bool {
-    int code = 0; unsigned long long h = 0; uint32_t koff = 0, klen = 0; bool ok = true;
+    int code = 0; uint32_t verr = 0; unsigned long long h = 0; uint32_t koff = 0, klen = 0; bool ok = true;
     if (lane < pend) {
       // entry: last key wins, values merge (same walk as decode.cuh parse_entry, without a schema)
       const uint8_t* key = nullptr;
       Cur c{my_ptr, my_ptr + my_len};
       FeatAcc acc; acc_reset(acc, K_NONE);
       int fl_code = -2;          // -2: no step seen yet
+      bool step_unset = false;   // a step whose kind is not set (the steps are typed in order: the first one throws)
       for (;;) {
         uint32_t tag;
         if (!rd_tag(c, tag)) { ok = false; break; }
@@ -98,7 +130,7 @@ __device__ __forceinline__ bool infer_map(const InferArgs& A, Cur body, bool is_
               if (!feature_scan(Cur{v.p, v.p + sl}, st, false, A.data)) { ok = false; break; }
               v.p += sl;
               int sc = feat_code(st);
-              if (sc < 0) { err = TFR_E_KIND_MISMATCH; }
+              if (sc < 0) step_unset = true;
               if (fl_code == -2) fl_code = sc; else if (sc > fl_code) fl_code = sc;      // reduceLeft(findTightestCommonType)
             }
             if (!ok) break;
@@ -108,19 +140,20 @@ __device__ __forceinline__ bool infer_map(const InferArgs& A, Cur body, bool is_
       if (ok) {
         h = hash64(key, klen);
         koff = key ? (uint32_t)(key - A.data) : 0;
-        if (!is_flist) { code = feat_code(acc); if (code < 0) err = TFR_E_KIND_MISMATCH; }
-        else if (fl_code == -2) { err = TFR_E_EMPTY_SCALAR; code = 0; }                 // empty.reduceLeft
+        if (!is_flist) { code = feat_code(acc); if (code < 0) { verr = INF_ERR_KIND; code = 0; } }
+        else if (fl_code == -2) verr = INF_ERR_EMPTY;                                   // empty.reduceLeft
+        else if (step_unset) verr = INF_ERR_KIND;
         else if (fl_code == 0) code = 10;                                               // ArrayType(ArrayType(null))
         else code = 7 + (fl_code - 1) % 3;                                              // T or [T] -> [[T]]
       }
     }
     if (__any_sync(FULLMASK, !ok)) return false;
-    if (lane < pend && klen >= (1u << 24)) atomicOr(&A.first_err[1], INF_OVF_KEY);
+    if (lane < pend && klen >= (1u << 24)) { atomicOr(&A.first_err[1], INF_OVF_KEY); over = true; }
     if (lane < pend && nent + lane < INFER_MAX_ENT) {
-      eh[nent + lane] = h; ecode[nent + lane] = (uint32_t)(code < 0 ? 0 : code) | (klen << 8); ekey[nent + lane] = koff;
+      eh[nent + lane] = h; ecode[nent + lane] = (uint32_t)code | (verr << 4) | (klen << 8); ekey[nent + lane] = koff;
     } else if (lane < pend) {
       // beyond the de-duplication window: last-wins cannot be decided any more
-      atomicOr(&A.first_err[1], INF_OVF_ENTRIES);
+      atomicOr(&A.first_err[1], INF_OVF_ENTRIES); over = true;
     }
     nent = min(nent + pend, (uint32_t)INFER_MAX_ENT);
     pend = 0;
@@ -142,6 +175,12 @@ __device__ __forceinline__ bool infer_map(const InferArgs& A, Cur body, bool is_
   return true;
 }
 
+// entries i and j of one map have the same key (the hash filters, the bytes decide)
+__device__ __forceinline__ bool same_key(const uint8_t* data, const unsigned long long* eh, const uint32_t* ecode, const uint32_t* ekey,
+                                         uint32_t i, uint32_t j) {
+  return eh[i] == eh[j] && (ecode[i] >> 8) == (ecode[j] >> 8) && bytes_equal(data + ekey[i], data + ekey[j], ecode[i] >> 8);
+}
+
 __global__ void __launch_bounds__(128) infer_kernel(InferArgs A) {
   extern __shared__ uint32_t smem[];
   uint32_t* stab = smem;
@@ -158,8 +197,10 @@ __global__ void __launch_bounds__(128) infer_kernel(InferArgs A) {
     const uint8_t* payload = A.data + off + 12;
     int err = 0;
     if (A.verify && crc_mask(crc_warp(stab, payload, len)) != load_u32_unaligned(payload + len)) err = TFR_E_CRC_DATA;
-    bool ok = true;
-    for (int pass = 0; pass < 2 && ok && !err; ++pass) {       // pass 0: features/context (field 1), pass 1: feature_lists (field 2)
+    bool ok = true, over = false;
+    uint32_t verr = 0;         // the record's first value error (INF_ERR_*): context's before feature_lists'
+    // pass 0: features/context (field 1), pass 1: feature_lists (field 2).  Both are parsed before a value error counts.
+    for (int pass = 0; pass < 2 && ok && !err; ++pass) {
       if (pass == 1 && A.record_type != TFR_RT_SEQUENCE_EXAMPLE) break;
       uint32_t nent = 0;
       Cur top{payload, payload + len};
@@ -170,25 +211,39 @@ __global__ void __launch_bounds__(128) infer_kernel(InferArgs A) {
         if (tag == 0x0A || (tag == 0x12 && A.record_type == TFR_RT_SEQUENCE_EXAMPLE)) {
           uint32_t l;
           if (!rd_len(top, l)) { ok = false; break; }
-          if ((tag == 0x0A) == (pass == 0) && !infer_map(A, Cur{top.p, top.p + l}, pass == 1, eh, ecode, ekey, nent, err)) { ok = false; break; }
+          if ((tag == 0x0A) == (pass == 0) && !infer_map(A, Cur{top.p, top.p + l}, pass == 1, eh, ecode, ekey, nent, over)) { ok = false; break; }
           top.p += l;
         } else if (!skip_field(top, tag)) { ok = false; break; }
       }
       if (!ok) break;
-      { uint32_t e = __reduce_max_sync(FULLMASK, err ? (uint32_t)(-err) : 0u); err = e ? -(int)e : 0; }
-      if (err) break;
       __syncwarp();
-      // Map.put semantics: an entry counts only if no later entry of this map has the same key
+      // Map.put semantics: an entry counts only if no later entry of this map has the same key; it sits at the position
+      // of the key's first occurrence, which orders the value errors
+      uint32_t first_err = 0xffffffffu;     // (first-occurrence position << 8) | INF_ERR_*
       for (uint32_t i = lane; i < nent; i += 32) {
         bool last = true;
-        for (uint32_t j = i + 1; j < nent; ++j) if (eh[j] == eh[i]) { last = false; break; }
-        if (last) infer_merge(A.table, eh[i], ekey[i], ecode[i] >> 8, (int)(ecode[i] & 0xff), &A.first_err[1]);
+        for (uint32_t j = i + 1; j < nent; ++j) if (same_key(A.data, eh, ecode, ekey, i, j)) { last = false; break; }
+        if (!last) continue;
+        const uint32_t e = (ecode[i] >> 4) & 0xf;
+        if (e) {
+          uint32_t pos = i;
+          for (uint32_t j = 0; j < i; ++j) if (same_key(A.data, eh, ecode, ekey, i, j)) { pos = j; break; }
+          first_err = min(first_err, (pos << 8) | e);
+        } else {
+          infer_merge(A.table, A.data, eh[i], ekey[i], ecode[i] >> 8, (int)(ecode[i] & 0xf), &A.first_err[1]);
+        }
       }
+      first_err = __reduce_min_sync(FULLMASK, first_err);
+      if (!verr && first_err != 0xffffffffu) verr = first_err & 0xff;
       __syncwarp();
     }
+    over = __any_sync(FULLMASK, over);
+    // a record that fails spoils the whole call, so what it merged into the table before failing is never read
     uint32_t st = 0;
     if (err) st = make_status(err, -1);
     else if (!ok) st = make_status(TFR_E_MALFORMED_PROTO, -1);
+    else if (over) { if (lane == 0) atomicMin(&A.first_err[4], row); }   // its entries past the window decide: unknown here
+    else if (verr) st = make_status(verr == INF_ERR_KIND ? TFR_E_KIND_MISMATCH : TFR_E_EMPTY_SCALAR, -1);
     if (lane == 0) { A.status[row] = st; if (st) atomicMin(&A.first_err[0], row); }
   }
 }
