@@ -39,11 +39,12 @@ static int32_t fail(int32_t code, const std::string& msg) { g_last_error = msg; 
     if (_e != cudaSuccess) return fail(TFR_E_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e)); \
   } while (0)
 
-int32_t DevBuf::ensure(size_t bytes) {
-  cudaError_t e = ensure_raw(bytes);
+static int32_t dev_alloc_status(cudaError_t e) {
   if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? TFR_E_OOM : TFR_E_CUDA, std::string("device allocation failed: ") + cudaGetErrorString(e));
   return TFR_OK;
 }
+int32_t DevBuf::ensure(size_t bytes) { return dev_alloc_status(ensure_raw(bytes)); }
+int32_t DevBuf::ensure_exact(size_t bytes) { return bytes <= cap ? TFR_OK : dev_alloc_status(alloc(bytes)); }
 #define TRY(expr) do { int32_t _rc = (expr); if (_rc) return _rc; } while (0)
 
 // NVTX range over one C-ABI call (SURVEY.md section 5: the tracing hook of this path)
@@ -158,15 +159,15 @@ static int32_t get_ctx(int device, DeviceCtx** out) {
     }
     // every handle's kernels read the tables from non-blocking streams, which are not ordered after the legacy default
     // stream: the copy is complete before any handle of this device exists
-    CrcTables* h = new CrcTables;
+    auto h = std::make_unique<CrcTables>();
     build_crc_tables(*h);
-    cudaStream_t st = nullptr;
-    c.err = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
+    Stream st;
+    c.err = st.create();
+    // a raw allocation on purpose: the tables live as long as the process.  g_ctx is static, and an owner's destructor would
+    // free them at exit, after the CUDA runtime has shut down.
     if (c.err == cudaSuccess) c.err = cudaMalloc(&c.d_tabs, sizeof(CrcTables));
-    if (c.err == cudaSuccess) c.err = cudaMemcpyAsync(c.d_tabs, h, sizeof(CrcTables), cudaMemcpyHostToDevice, st);
+    if (c.err == cudaSuccess) c.err = cudaMemcpyAsync(c.d_tabs, h.get(), sizeof(CrcTables), cudaMemcpyHostToDevice, st);
     if (c.err == cudaSuccess) c.err = cudaStreamSynchronize(st);
-    if (st) cudaStreamDestroy(st);
-    delete h;
   });
   if (c.err != cudaSuccess) return fail(TFR_E_CUDA, std::string("device init: ") + cudaGetErrorString(c.err));
   *out = &c;
@@ -193,7 +194,7 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
   if (record_type < TFR_RT_EXAMPLE || record_type > TFR_RT_BYTE_ARRAY)
     return fail(TFR_E_BAD_RECORD_TYPE, "Unsupported recordType: recordType can be ByteArray, Example or SequenceExample");
   if (n_fields > 4096) return fail(TFR_E_INVALID_ARG, "more than 4096 fields");
-  auto* s = new tfr_schema;
+  auto s = std::make_unique<tfr_schema>();
   s->record_type = record_type;
   if (record_type == TFR_RT_BYTE_ARRAY) {
     // the single binary column of TensorFlowInferSchema.getSchemaForByteArray (M/TensorFlowInferSchema.scala:60-64);
@@ -208,18 +209,18 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
     s->n_var = 1; s->n_cnt = 1;
     s->ht.assign(2, -1);
     s->ht[d.hash & 1] = 0;
-    *out = s;
+    *out = s.release();
     return TFR_OK;
   }
   for (int32_t i = 0; i < n_fields; ++i) {
     const tfr_field& f = fields[i];
-    if (f.name_len < 0 || (f.name_len > 0 && !f.name)) { delete s; return fail(TFR_E_INVALID_ARG, "bad field name"); }
+    if (f.name_len < 0 || (f.name_len > 0 && !f.name)) return fail(TFR_E_INVALID_ARG, "bad field name");
     std::string nm(f.name ? f.name : "", (size_t)f.name_len);
     // newFeatureWriter / newFeatureConverter: anything but these types throws (M/TFRecordDeserializer.scala:119-123,
     // M/TFRecordSerializer.scala:147,151); ArrayType(NullType) falls into the same default branch
     bool ok_type = f.elem_type >= TFR_T_NULL && f.elem_type <= TFR_T_BINARY && f.depth >= 0 && f.depth <= 2 &&
                    !(f.elem_type == TFR_T_NULL && f.depth > 0);
-    if (!ok_type) { delete s; return fail(TFR_E_UNSUPPORTED_TYPE, "field '" + nm + "': data type is not supported"); }
+    if (!ok_type) return fail(TFR_E_UNSUPPORTED_TYPE, "field '" + nm + "': data type is not supported");
     DevField d{};
     d.name_off = (uint32_t)s->names.size();
     d.name_len = (uint32_t)f.name_len;
@@ -246,14 +247,13 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
     size_t slot = d.hash & (hsz - 1);
     while (s->ht[slot] >= 0) {
       const DevField& o = s->fields[s->ht[slot]];
-      if (o.hash == d.hash && o.name_len == d.name_len && memcmp(&s->names[o.name_off], &s->names[d.name_off], d.name_len) == 0) {
-        delete s; return fail(TFR_E_INVALID_ARG, "Found duplicate column(s) in the data schema");
-      }
+      if (o.hash == d.hash && o.name_len == d.name_len && memcmp(&s->names[o.name_off], &s->names[d.name_off], d.name_len) == 0)
+        return fail(TFR_E_INVALID_ARG, "Found duplicate column(s) in the data schema");
       slot = (slot + 1) & (hsz - 1);
     }
     s->ht[slot] = i;
   }
-  *out = s;
+  *out = s.release();
   return TFR_OK;
 }
 extern "C" void tfr_schema_destroy(tfr_schema* s) { delete s; }
@@ -262,20 +262,21 @@ extern "C" int32_t tfr_schema_num_fields(const tfr_schema* s) { return s ? (int3
 // device copy of a schema.  The copies run on the handle's stream `st` and are waited for before returning: the handle's
 // kernels run on non-blocking streams, which nothing orders after the legacy default stream, and `tp` is a local.
 struct DevSchemaBuf {
-  DevField* d_fields = nullptr; uint8_t* d_names = nullptr; int32_t* d_ht = nullptr; int32_t* d_var_field = nullptr;
-  FieldTemplate* d_templates = nullptr;
-  uint8_t* d_tile_consts = nullptr; uint32_t tile_consts_bytes = 0;     // tile.cuh: per-schema constants in the shared-memory layout
+  DevBuf fields, names, ht, var_field, templates;
+  DevBuf tile_consts; uint32_t tile_consts_bytes = 0;     // tile.cuh: per-schema constants in the shared-memory layout
   DevSchema view{};
+  const int32_t* d_var_field() const { return (const int32_t*)var_field.p; }
+  const uint8_t* d_tile_consts() const { return (const uint8_t*)tile_consts.p; }
   int32_t upload(const tfr_schema& s, cudaStream_t st) {
     size_t nf = s.fields.size();
-    CUDA_TRY(cudaMalloc(&d_fields, std::max<size_t>(1, nf) * sizeof(DevField)));
-    CUDA_TRY(cudaMalloc(&d_names, std::max<size_t>(1, s.names.size())));
-    CUDA_TRY(cudaMalloc(&d_ht, s.ht.size() * sizeof(int32_t)));
-    CUDA_TRY(cudaMalloc(&d_var_field, std::max<size_t>(1, s.var_field.size()) * sizeof(int32_t)));
-    if (nf) CUDA_TRY(cudaMemcpyAsync(d_fields, s.fields.data(), nf * sizeof(DevField), cudaMemcpyHostToDevice, st));
-    if (!s.names.empty()) CUDA_TRY(cudaMemcpyAsync(d_names, s.names.data(), s.names.size(), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_ht, s.ht.data(), s.ht.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    if (!s.var_field.empty()) CUDA_TRY(cudaMemcpyAsync(d_var_field, s.var_field.data(), s.var_field.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(fields.alloc(std::max<size_t>(1, nf) * sizeof(DevField)));
+    CUDA_TRY(names.alloc(std::max<size_t>(1, s.names.size())));
+    CUDA_TRY(ht.alloc(s.ht.size() * sizeof(int32_t)));
+    CUDA_TRY(var_field.alloc(std::max<size_t>(1, s.var_field.size()) * sizeof(int32_t)));
+    if (nf) CUDA_TRY(cudaMemcpyAsync(fields.p, s.fields.data(), nf * sizeof(DevField), cudaMemcpyHostToDevice, st));
+    if (!s.names.empty()) CUDA_TRY(cudaMemcpyAsync(names.p, s.names.data(), s.names.size(), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ht.p, s.ht.data(), s.ht.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    if (!s.var_field.empty()) CUDA_TRY(cudaMemcpyAsync(var_field.p, s.var_field.data(), s.var_field.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     {
       // canonical entry prefix of every field: 0A ? 0A klen key 12 ? kindtag ?   (? = length bytes, masked out)
       std::vector<FieldTemplate> tp(std::max<size_t>(1, nf));
@@ -295,33 +296,32 @@ struct DevSchemaBuf {
         t.n_words = (uint16_t)((total + 3) / 4); t.klen = (uint16_t)klen;
         memcpy(t.words, bytes, sizeof bytes); memcpy(t.mask, mask, sizeof mask);
       }
-      CUDA_TRY(cudaMalloc(&d_templates, tp.size() * sizeof(FieldTemplate)));
-      CUDA_TRY(cudaMemcpyAsync(d_templates, tp.data(), tp.size() * sizeof(FieldTemplate), cudaMemcpyHostToDevice, st));
+      CUDA_TRY(templates.alloc(tp.size() * sizeof(FieldTemplate)));
+      CUDA_TRY(cudaMemcpyAsync(templates.p, tp.data(), tp.size() * sizeof(FieldTemplate), cudaMemcpyHostToDevice, st));
       CUDA_TRY(cudaStreamSynchronize(st));
     }
     view.n_fields = (int32_t)nf; view.record_type = s.record_type; view.ht_mask = (int32_t)s.ht.size() - 1;
     view.n_fix = s.n_fix; view.n_var = s.n_var; view.n_cnt = s.n_cnt;
-    view.fields = d_fields; view.names = d_names; view.ht = d_ht;
+    view.fields = (DevField*)fields.p; view.names = (uint8_t*)names.p; view.ht = (int32_t*)ht.p;
     return TFR_OK;
   }
   // CRC tables | zeroed seen words | DevField[nf] | FieldTemplate[nf] | names, each section 16-byte aligned (tile_const_bytes)
   int32_t build_tile_consts(const tfr_schema& s, const CrcTables* d_tabs, cudaStream_t st) {
     const uint32_t nf = (uint32_t)s.fields.size(), nb = (uint32_t)s.names.size();
     tile_consts_bytes = tile_const_bytes(nf, nb);
-    CUDA_TRY(cudaMalloc(&d_tile_consts, tile_consts_bytes));
-    CUDA_TRY(cudaMemsetAsync(d_tile_consts, 0, tile_consts_bytes, st));
-    uint8_t* q = d_tile_consts;
+    CUDA_TRY(tile_consts.alloc(tile_consts_bytes));
+    CUDA_TRY(cudaMemsetAsync(tile_consts.p, 0, tile_consts_bytes, st));
+    uint8_t* q = (uint8_t*)tile_consts.p;
     CUDA_TRY(cudaMemcpyAsync(q, d_tabs->g5, TILE_CRC_BYTES, cudaMemcpyDeviceToDevice, st));   // g5 then xp16, contiguous in CrcTables
     q += TILE_CRC_BYTES + TILE_SEEN_BYTES;
-    if (nf) CUDA_TRY(cudaMemcpyAsync(q, d_fields, nf * sizeof(DevField), cudaMemcpyDeviceToDevice, st));
+    if (nf) CUDA_TRY(cudaMemcpyAsync(q, fields.p, nf * sizeof(DevField), cudaMemcpyDeviceToDevice, st));
     q += (nf * sizeof(DevField) + 15) & ~(size_t)15;
-    if (nf) CUDA_TRY(cudaMemcpyAsync(q, d_templates, nf * sizeof(FieldTemplate), cudaMemcpyDeviceToDevice, st));
+    if (nf) CUDA_TRY(cudaMemcpyAsync(q, templates.p, nf * sizeof(FieldTemplate), cudaMemcpyDeviceToDevice, st));
     q += (nf * sizeof(FieldTemplate) + 15) & ~(size_t)15;
-    if (nb) CUDA_TRY(cudaMemcpyAsync(q, d_names, nb, cudaMemcpyDeviceToDevice, st));
+    if (nb) CUDA_TRY(cudaMemcpyAsync(q, names.p, nb, cudaMemcpyDeviceToDevice, st));
     CUDA_TRY(cudaStreamSynchronize(st));             // the decoder's kernels read these from its other streams too
     return TFR_OK;
   }
-  void free_all() { cudaFree(d_fields); cudaFree(d_names); cudaFree(d_ht); cudaFree(d_var_field); cudaFree(d_templates); cudaFree(d_tile_consts); }
 };
 
 // Raises Kernel's opt-in dynamic shared memory to at least `smem` bytes on the current device; never lowers it.

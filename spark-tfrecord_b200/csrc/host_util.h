@@ -1,33 +1,107 @@
-// host_util.h -- small host-side helpers for api.cu: growable device buffers, a pinned host block
-// pool, and the Arrow C Data / Device Interface structs (restated from the Arrow ABI specification,
-// identical in layout to arrow/c/abi.h).
+// host_util.h -- host-side helpers for api.cu: the owners of every CUDA resource a handle holds (device buffers, pinned host
+// buffers, streams, events, the block pools), and the Arrow C Data / Device Interface structs (restated from the Arrow ABI
+// specification, identical in layout to arrow/c/abi.h).
+//
+// This file is the only place that calls the raw allocate / free / create / destroy functions of the CUDA runtime.  Each
+// owner frees what it holds in its destructor, without waiting: a handle synchronises its streams before its members go (a
+// pending copy may still use a pinned mirror).  No owner may live in static storage, where its destructor would run after
+// the CUDA runtime has shut down at exit.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <memory>
+#include <utility>
 #include <vector>
 
-struct DevBuf {
+// a block of device memory (cudaMalloc) or of pinned host memory (cudaHostAlloc)
+template <bool Pinned>
+struct MemBlock {
   void* p = nullptr;
   size_t cap = 0;
-  // grows (never shrinks); contents are NOT preserved
-  cudaError_t ensure_raw(size_t bytes) {
-    if (bytes <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr; cap = 0;
-    size_t want = bytes + bytes / 4 + 256;
-    cudaError_t e = cudaMalloc(&p, want);
-    if (e != cudaSuccess) { e = cudaMalloc(&p, bytes); want = bytes; }
-    if (e == cudaSuccess) cap = want;
+  MemBlock() = default;
+  MemBlock(MemBlock&& o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+  MemBlock& operator=(MemBlock&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
+  ~MemBlock() { reset(); }
+  // replaces the block by one of exactly `bytes`; contents are NOT preserved, empty on failure
+  cudaError_t alloc(size_t bytes) {
+    reset();
+    cudaError_t e = Pinned ? cudaHostAlloc(&p, bytes, cudaHostAllocDefault) : cudaMalloc(&p, bytes);
+    if (e == cudaSuccess) cap = bytes; else p = nullptr;
     return e;
   }
-  int32_t ensure(size_t bytes);
-  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+ private:
+  void reset() { if (p) { if (Pinned) cudaFreeHost(p); else cudaFree(p); } p = nullptr; cap = 0; }
+};
+
+// pinned host memory.  The caller decides when it grows and to what size (each use has its own rounding).
+using PinnedBuf = MemBlock<true>;
+
+// device memory
+struct DevBuf : MemBlock<false> {
+  // grows (never shrinks) to at least `bytes`, with a quarter of head-room when that fits; contents are NOT preserved
+  cudaError_t ensure_raw(size_t bytes) {
+    if (bytes <= cap) return cudaSuccess;
+    cudaError_t e = alloc(bytes + bytes / 4 + 256);
+    return e == cudaSuccess ? e : alloc(bytes);
+  }
+  int32_t ensure(size_t bytes);          // ensure_raw; a failure is reported through tfr_last_error (api.cu)
+  int32_t ensure_exact(size_t bytes);    // grows (never shrinks) to exactly `bytes`; a failure is reported as ensure's
+};
+
+// a non-blocking stream; null until created
+class Stream {
+  cudaStream_t s_ = nullptr;
+ public:
+  Stream() = default;
+  Stream(Stream&& o) noexcept : s_(std::exchange(o.s_, nullptr)) {}
+  Stream& operator=(Stream&& o) noexcept { std::swap(s_, o.s_); return *this; }
+  ~Stream() { if (s_) cudaStreamDestroy(s_); }
+  cudaError_t create() { return cudaStreamCreateWithFlags(&s_, cudaStreamNonBlocking); }
+  cudaError_t create(int priority) { return cudaStreamCreateWithPriority(&s_, cudaStreamNonBlocking, priority); }
+  // waits for the stream's work.  A stream never created is skipped: synchronising the null stream would wait for the legacy
+  // default stream, and so for other threads' work.
+  void sync() const { if (s_) cudaStreamSynchronize(s_); }
+  operator cudaStream_t() const { return s_; }
+};
+
+// an event without timing; null until created
+class Event {
+  cudaEvent_t e_ = nullptr;
+ public:
+  Event() = default;
+  Event(Event&& o) noexcept : e_(std::exchange(o.e_, nullptr)) {}
+  Event& operator=(Event&& o) noexcept { std::swap(e_, o.e_); return *this; }
+  ~Event() { if (e_) cudaEventDestroy(e_); }
+  cudaError_t create() { return cudaEventCreateWithFlags(&e_, cudaEventDisableTiming); }
+  operator cudaEvent_t() const { return e_; }
+};
+
+// Events lent out and taken back (a batch's completion, a profiling span's ends).  The pool owns every event it ever
+// created; borrowers hold plain handles and never destroy them.
+class EventPool {
+  unsigned flags_;
+  std::vector<cudaEvent_t> all_, free_;
+ public:
+  explicit EventPool(unsigned flags) : flags_(flags) {}
+  EventPool(const EventPool&) = delete;
+  EventPool& operator=(const EventPool&) = delete;
+  ~EventPool() { for (cudaEvent_t e : all_) cudaEventDestroy(e); }
+  cudaError_t take(cudaEvent_t* out) {
+    if (!free_.empty()) { *out = free_.back(); free_.pop_back(); return cudaSuccess; }
+    cudaEvent_t e = nullptr;
+    cudaError_t err = cudaEventCreateWithFlags(&e, flags_);
+    if (err == cudaSuccess) { all_.push_back(e); *out = e; }
+    return err;
+  }
+  void give(cudaEvent_t e) { if (e) free_.push_back(e); }
 };
 
 struct PinnedPool {
   struct Block { void* p; size_t cap; bool used; };
   std::vector<Block> blocks;
+  PinnedPool() = default;
+  PinnedPool(const PinnedPool&) = delete;
+  PinnedPool& operator=(const PinnedPool&) = delete;
+  ~PinnedPool() { for (auto& b : blocks) cudaFreeHost(b.p); }
   void* acquire(size_t bytes) {
     int best = -1;
     for (size_t i = 0; i < blocks.size(); ++i)
@@ -44,7 +118,6 @@ struct PinnedPool {
     return p;
   }
   void give_back(void* p) { for (auto& b : blocks) if (b.p == p) b.used = false; }
-  void release_all() { for (auto& b : blocks) cudaFreeHost(b.p); blocks.clear(); }
 };
 
 // device blocks reused across batches.  A block goes back to the pool when its batch is released, possibly while kernels that
@@ -55,6 +128,10 @@ struct DevPool {
   struct Block { void* p; size_t cap; bool used; cudaEvent_t ready; unsigned long long stamp; };
   std::vector<Block> blocks;
   unsigned long long clock = 0;
+  DevPool() = default;
+  DevPool(const DevPool&) = delete;
+  DevPool& operator=(const DevPool&) = delete;
+  ~DevPool() { for (auto& b : blocks) { cudaFree(b.p); if (b.ready) cudaEventDestroy(b.ready); } }
   void* acquire(size_t bytes, cudaEvent_t* ready_out = nullptr) {
     int best = -1;
     for (size_t i = 0; i < blocks.size(); ++i) {
@@ -87,7 +164,6 @@ struct DevPool {
         if (b.ready) cudaEventRecord(b.ready, st);
       }
   }
-  void release_all() { for (auto& b : blocks) { cudaFree(b.p); if (b.ready) cudaEventDestroy(b.ready); } blocks.clear(); }
 };
 
 extern "C" {

@@ -4,7 +4,8 @@ Spark runs several tasks per executor, each with its own decoder, encoder or inf
 handle's work runs on non-blocking streams.  A non-blocking stream has no ordering with the legacy default stream, so device
 state a kernel reads must be written on the handle's own stream and waited for; and the opt-in shared-memory attribute of a
 kernel is process-wide, so raising it is a check-then-set that must not race (DESIGN.md section 4, INTEGRATION.md
-"Threading/ownership")."""
+"Threading/ownership").  A task retried after an allocation failure must not leak what its handle had built, so every CUDA
+resource has an owner type whose destructor frees it (DESIGN.md section 3)."""
 import os
 import re
 
@@ -27,6 +28,17 @@ def _calls(code, name):
             depth += {"(": 1, ")": -1}.get(code[i], 0)
             i += 1
         yield code.count("\n", 0, m.start()) + 1, code[m.end():i - 1]
+
+
+def _braced_body(code, header):
+    """(offset, text) of the brace-matched body that follows the regex `header` (which ends at the opening brace)"""
+    m = re.search(header, code)
+    assert m, f"{header} not found"
+    depth, i = 1, m.end()
+    while depth:
+        depth += {"{": 1, "}": -1}.get(code[i], 0)
+        i += 1
+    return m.end(), code[m.end():i]
 
 
 def _last_arg(args):
@@ -79,16 +91,32 @@ def test_raise_dyn_smem_checks_and_sets_under_a_lock():
         sets += [(f, ln) for ln, args in _calls(code, "cudaFuncSetAttribute") if "MaxDynamicSharedMemorySize" in args]
     assert len(sets) == 1, f"every opt-in raise goes through raise_dyn_smem: {sets}"
     code = dict(_sources())["api.cu"]
-    m = re.search(r"static\s+cudaError_t\s+raise_dyn_smem\s*\([^)]*\)\s*\{", code)
-    assert m, "raise_dyn_smem not found in api.cu"
-    depth, i = 1, m.end()
-    while depth:
-        depth += {"{": 1, "}": -1}.get(code[i], 0)
-        i += 1
-    body = code[m.end():i]
+    _, body = _braced_body(code, r"static\s+cudaError_t\s+raise_dyn_smem\s*\([^)]*\)\s*\{")
     assert "cudaFuncSetAttribute" in body
     lock = re.search(r"std::(lock_guard|unique_lock|scoped_lock)\s*<\s*std::mutex\s*>", body)
     assert lock, "raise_dyn_smem takes no lock"
     before_set = body[lock.end():body.index("cudaFuncSetAttribute")]
     assert "granted" in before_set, "the size is checked again under the lock, before the attribute is set"
     assert re.search(r"std::atomic\s*<\s*size_t\s*>\s+granted", body), "the unlocked fast path reads an atomic"
+
+
+def test_cuda_resources_are_allocated_and_freed_only_by_their_owners():
+    """Every device buffer, pinned host buffer, stream and event of a handle is held by an owner type of host_util.h whose
+    destructor frees it, so a create function that returns early frees whatever it had built.  Outside host_util.h nothing
+    allocates, frees, creates or destroys one by hand.  The one exception is the device copy of the CRC tables in get_ctx:
+    it lives as long as the process, in static storage, where a destructor would run after the CUDA runtime has shut down."""
+    raw = re.compile(r"\b(cuda(?:Malloc|Free|HostAlloc|StreamCreate|StreamDestroy|EventCreate|EventDestroy)\w*)\s*\(")
+    api = dict(_sources())["api.cu"]
+    start, body = _braced_body(api, r"static\s+int32_t\s+get_ctx\s*\([^)]*\)\s*\{")
+    bad, allowed = [], []
+    for f, code in _sources():
+        if f == "host_util.h":
+            continue
+        for m in raw.finditer(code):
+            where = f"{f}:{code.count(chr(10), 0, m.start()) + 1}: {m.group(1)}("
+            if f == "api.cu" and m.group(1) == "cudaMalloc" and start <= m.start() < start + len(body):
+                allowed.append(where)
+            else:
+                bad.append(where)
+    assert not bad, "raw CUDA allocations / frees outside the owners of host_util.h:\n" + "\n".join(bad)
+    assert len(allowed) == 1, f"get_ctx allocates the CRC tables once: {allowed}"
