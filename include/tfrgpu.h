@@ -165,8 +165,10 @@ int32_t tfr_decoder_get_profile(tfr_decoder*, double* ms /* [TFR_PROFILE_STAGES]
 /* counters since creation: [0] batches decoded, [1] submitted speculatively (no host sync), [2] of those redone after
  * the device raised a flag, [3] batches through count mode (ragged / learning), [4] through the general kernels,
  * [5] column shapes (re)learned, [6] batches re-run by the single-pass kernel's transcoding instantiation (malformed
- * UTF-8 in a string column)                                                                                       */
-int32_t tfr_decoder_get_stats(tfr_decoder*, int64_t* out, int32_t n /* <= 8 */);
+ * UTF-8 in a string column), [7] rows passes enqueued by tfr_batch_rows_async without a host synchronisation, [8] of
+ * those rebuilt through the synchronous rows path (the batch was redone, or the rows did not fit what they were
+ * launched with).  A caller passing n = 8 gets the first eight.                                                   */
+int32_t tfr_decoder_get_stats(tfr_decoder*, int64_t* out, int32_t n /* <= 10 */);
 
 int32_t tfr_batch_wait(tfr_batch*);
 typedef struct tfr_batch_info {
@@ -294,6 +296,38 @@ int32_t tfr_batch_rows(tfr_batch*, int32_t to_host, const void** rows, const int
 int32_t tfr_batch_rows_with_partition(tfr_batch*, int32_t to_host, const void* part_row, size_t part_row_bytes,
                                       int32_t n_part_fields, const uint8_t* part_var, const void** rows,
                                       const int64_t** row_offsets, int64_t* n_rows, size_t* nbytes);
+
+/* ---- pipelined rows of a decoded batch ---------------------------------------------------
+ * tfr_batch_rows_async enqueues, behind the batch's kernels, the rows pass tfr_batch_rows_with_partition would run with the
+ * same arguments (np = 0, part_row = part_var = NULL: tfr_batch_rows), and with to_host = 1 also their copy into pinned host
+ * memory owned by the batch, and returns without waiting.  It may be called right after tfr_decode_submit, before
+ * tfr_batch_consumed: a streaming reader then has the rows and their copy of block k queued behind its decode while it
+ * submits block k+1, and its rows call for block k finds them done.
+ *   Reading      : the rows are read with tfr_batch_rows / tfr_batch_rows_with_partition, whose bytes, offsets, n_rows and
+ *                  nbytes are byte-identical to what they return without the asynchronous call, for either to_host (0 after
+ *                  an asynchronous call gives the device rows; 1 after an asynchronous to_host = 0 adds only the copy).
+ *   Partition    : the asynchronous call counts as the build: a later call with another partition row gets
+ *                  TFR_E_INVALID_ARG, and the rows already asked for stay valid.  A second asynchronous call with the same
+ *                  arguments, or one after the rows were built, does nothing (except that to_host = 1 after an asynchronous
+ *                  to_host = 0 enqueues the copy).
+ *   Errors       : returned at once are only the argument errors tfr_batch_rows_with_partition checks before any work (a
+ *                  null batch, every partition-row case listed above, a DecimalType data field as TFR_E_UNSUPPORTED_TYPE
+ *                  naming the field, the batch staying usable for columns), and TFR_E_OOM / TFR_E_CUDA.  A row above
+ *                  INT32_MAX bytes (TFR_E_BATCH_TOO_LARGE) is reported by the later rows call, exactly as without it.
+ *   Synchronisation : a decoder learns its row sizes from the first clean batch of more than 64 rows whose rows it builds,
+ *                  on either path.  Before that the asynchronous call only records the request, and the rows call builds
+ *                  the rows as it would without it.  After it, every asynchronous call enqueues with no host
+ *                  synchronisation, for pipelined batches and for batches decoded synchronously alike.  The rows block is
+ *                  sized from the learned data-row bytes per framed byte plus head-room, plus the partition bytes of every
+ *                  row the batch can hold.
+ *   Redo         : rows enqueued for a batch that is later redone (its pipelined decode raised a flag), or whose device
+ *                  verdict says they did not fit what they were launched with, are dropped, and the rows call rebuilds them
+ *                  through the synchronous path.  The caller never sees a speculative row.
+ *   Release      : tfr_batch_release of a batch with rows enqueued waits for them before its buffers go back to the
+ *                  decoder, as it does for built rows.
+ * tfr_decoder_get_stats counts the passes enqueued ([7]) and those rebuilt ([8]).                                        */
+int32_t tfr_batch_rows_async(tfr_batch*, int32_t to_host, const void* part_row, size_t part_row_bytes,
+                             int32_t n_part_fields, const uint8_t* part_var);
 
 /* ---- encode: replaces TFRecordOutputWriter.write/close -------------------------------- */
 /* Replaces the constructor M/TFRecordOutputWriter.scala:12-24.                             */

@@ -25,7 +25,7 @@ EXPORTS = [
     "tfr_decoder_num_staging_slots", "tfr_decode", "tfr_decode_submit",
     "tfr_decoder_stream", "tfr_decoder_set_profiling", "tfr_decoder_get_profile", "tfr_decoder_get_stats", "tfr_batch_wait", "tfr_batch_status", "tfr_batch_consumed", "tfr_batch_num_columns", "tfr_batch_columns",
     "tfr_batch_to_host_async", "tfr_batch_to_host", "tfr_batch_export_arrow_host", "tfr_batch_export_arrow_device", "tfr_batch_release",
-    "tfr_batch_rows", "tfr_batch_rows_with_partition",
+    "tfr_batch_rows", "tfr_batch_rows_with_partition", "tfr_batch_rows_async",
     "tfr_encoder_create", "tfr_encoder_destroy", "tfr_encode", "tfr_encoder_row_staging", "tfr_encode_rows", "tfr_encoder_result_host",
     "tfr_encoder_stream", "tfr_encoder_num_row_slots", "tfr_encoder_row_staging_slot", "tfr_encode_rows_submit", "tfr_encoded_wait",
     "tfr_encoded_result", "tfr_encoded_release", "tfr_encoder_get_stats",
@@ -128,6 +128,7 @@ def lib():
         "tfr_batch_release": (None, [vp]),
         "tfr_batch_rows": (i32, [vp, i32, P(vp), P(vp), P(i64), P(sz)]),
         "tfr_batch_rows_with_partition": (i32, [vp, i32, vp, sz, i32, vp, P(vp), P(vp), P(i64), P(sz)]),
+        "tfr_batch_rows_async": (i32, [vp, i32, vp, sz, i32, vp]),
         "tfr_encoder_create": (i32, [vp, i32, u32, P(vp)]),
         "tfr_encoder_destroy": (None, [vp]),
         "tfr_encode": (i32, [vp, P(tfr_column), i32, i32, P(vp), P(sz), P(i64)]),
@@ -285,6 +286,15 @@ class Batch:
         offs = np.ctypeslib.as_array(C.cast(op, C.POINTER(C.c_int64)), shape=(n.value + 1,))
         return rows, offs
 
+    def unsafe_rows_async(self, to_host: bool = True, partition=None):
+        """Enqueue the rows unsafe_rows() returns, and with to_host their copy to pinned memory, behind the batch's kernels
+        without waiting (tfr_batch_rows_async); unsafe_rows() then reads them.  partition as in unsafe_rows()."""
+        if partition is None:
+            _check(lib().tfr_batch_rows_async(self.h, 1 if to_host else 0, None, 0, 0, None))
+        else:
+            row, flags = bytes(partition[0]), bytes(bytearray(partition[1]))
+            _check(lib().tfr_batch_rows_async(self.h, 1 if to_host else 0, row, len(row), len(flags), flags))
+
     def raise_if_error(self):
         if self.info["error_code"]:
             raise error_for(self.info["error_code"], "", self.info["error_row"], self.info["error_field"])
@@ -326,9 +336,10 @@ class Decoder:
         return lib().tfr_decoder_num_staging_slots()
 
     def stats(self) -> dict:
-        v = (C.c_int64 * 8)()
-        _check(lib().tfr_decoder_get_stats(self.h, v, 8))
-        names = ["batches", "speculative_submits", "speculative_redone", "count_mode_batches", "general_path_batches", "shapes_learned", "transcode_reruns"]
+        v = (C.c_int64 * 10)()
+        _check(lib().tfr_decoder_get_stats(self.h, v, 10))
+        names = ["batches", "speculative_submits", "speculative_redone", "count_mode_batches", "general_path_batches", "shapes_learned", "transcode_reruns",
+                 "rows_async", "rows_async_rebuilt"]
         return {k: v[i] for i, k in enumerate(names)}
 
     def stream(self) -> int:

@@ -21,6 +21,13 @@
 //                       small table in global memory that every CTA reads (L1 / L2 hits after the first).
 // Only the batch's column buffers and this pass's own scratch are read.
 //
+// tfr_batch_rows_async enqueues the same pass before the batch's row count is known on the host (api_decode.inc): the size
+// kernel's CAP instantiation runs over the batch's row CAPACITY and reads the true count from the control words (UrCtl) in
+// device memory, the scans run over the capacity unchanged (so every offset from the count on equals the total),
+// urows_verdict_kernel checks what the host could not (the decode's verdict, the rows block's capacity, a too-large row), and
+// the emit kernel's GUARD instantiation does nothing once the verdict is raised.  The host then rebuilds the rows through the
+// synchronous path.  CAP = false and GUARD = false are the kernels tfr_batch_rows launches; they never read the control words.
+//
 // Reference semantics: what Spark's UnsafeProjection makes of the SpecificInternalRow TFRecordDeserializer fills
 // (M/TFRecordDeserializer.scala:21-61): the published UnsafeRow / UnsafeArrayData layout.
 #pragma once
@@ -62,6 +69,11 @@ struct UrArgs {
   uint32_t smem_cap;            // tile bytes the shared-memory staging holds
 };
 
+// control words of the rows pass (uint32, in its scratch): the too-large row and the scan overflow are those of tfr_batch_rows;
+// the asynchronous pass adds the row count and the decode flags it was given (copied from the decode's result block, or
+// written by the host), the verdict, and the total bytes
+enum { URC_TOO_LARGE = 0, URC_OVERFLOW = 1, URC_N = 2, URC_DFLAGS = 3, URC_VERDICT = 4, URC_TOTAL = 6, URC_WORDS = 8 };
+
 __device__ __forceinline__ uint64_t ur_pad8(uint64_t v) { return (v + 7) & ~7ull; }
 __device__ __forceinline__ uint64_t ur_hdr(uint64_t n) { return 8 + (n + 63) / 64 * 8; }     // numElements + element null bitset
 
@@ -89,9 +101,17 @@ __device__ __forceinline__ bool ur_present(const UrCol& c, uint32_t r) {
   return c.kind != UR_NULL && ((c.valid[r >> 5] >> (r & 31)) & 1u);
 }
 
-__global__ void __launch_bounds__(UROWS_SIZE_THREADS) urows_size_kernel(UrArgs A) {
+// CAP: launched over the row capacity A.n_rows (the stride of `pos`); rows at or beyond ctl[URC_N] get size 0 and read no column
+// memory (a speculative batch's offsets past its count are garbage), and so does every row when the decode raised a flag or
+// counted more rows than the capacity.  CAP = false never reads `ctl`.
+template <bool CAP>
+__global__ void __launch_bounds__(UROWS_SIZE_THREADS) urows_size_kernel(UrArgs A, const uint32_t* ctl) {
   const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= A.n_rows) return;
+  if (CAP) {
+    const uint32_t n = ctl[URC_N];
+    if (ctl[URC_DFLAGS] || n > A.n_rows || r >= n) { A.size[r] = 0u; return; }
+  }
   uint64_t s = 8ull * (A.nw + A.nf + A.np);
   for (uint32_t f = 0; f < A.nf; ++f) {
     const UrCol& c = A.cols[f];
@@ -195,10 +215,26 @@ __device__ void ur_emit_lane(const UrCol& c, uint32_t r, uint8_t* dst) {
   }
 }
 
-__global__ void __launch_bounds__(UROWS_WARPS * 32) urows_emit_kernel(UrArgs A) {
+// After the scan, one thread: raises ctl[URC_VERDICT] when the rows the asynchronous pass built cannot be handed out -- the
+// decode raised a flag or counted more rows than its capacity `n_alloc` (the batch is redone), the rows need more than the
+// `rows_cap` bytes of their block, or a row is larger than INT32_MAX bytes -- and stores the total at ctl[URC_TOTAL].
+__global__ void urows_verdict_kernel(uint32_t* ctl, const uint64_t* total, uint32_t n_alloc, unsigned long long rows_cap) {
+  const uint64_t t = *total;
+  const bool bad = ctl[URC_DFLAGS] != 0u || ctl[URC_N] > n_alloc || t > rows_cap || ctl[URC_TOO_LARGE] != 0xffffffffu;
+  ctl[URC_VERDICT] = bad ? 1u : 0u;
+  *reinterpret_cast<unsigned long long*>(ctl + URC_TOTAL) = t;
+}
+
+// GUARD: the asynchronous pass's instantiation.  It returns at once when urows_verdict_kernel has raised the verdict, takes the
+// row count from ctl[URC_N] (A.n_rows is the capacity, the stride of `pos`), and CTAs past the count exit.  GUARD = false never
+// reads `ctl`.
+template <bool GUARD>
+__global__ void __launch_bounds__(UROWS_WARPS * 32) urows_emit_kernel(UrArgs A, const uint32_t* ctl) {
   extern __shared__ __align__(16) uint8_t ur_smem[];
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const uint32_t r0 = blockIdx.x * UROWS_TILE, rows = min((uint32_t)UROWS_TILE, A.n_rows - r0);
+  const uint32_t n_rows = GUARD ? ctl[URC_N] : A.n_rows;
+  if (GUARD && (ctl[URC_VERDICT] || blockIdx.x * UROWS_TILE >= n_rows)) return;
+  const uint32_t r0 = blockIdx.x * UROWS_TILE, rows = min((uint32_t)UROWS_TILE, n_rows - r0);
   const int64_t t_lo = A.offs[r0], t_hi = A.offs[r0 + rows];
   const uint64_t span = (uint64_t)(t_hi - t_lo);
   const uint32_t phase = (uint32_t)(t_lo & 15);                   // smem keeps the output's 16-byte phase: 16-byte stores out

@@ -21,6 +21,9 @@
 //     static native java.nio.ByteBuffer[] batchRows(long batch);   // {rows, int64 row offsets}: pinned UnsafeRows, valid until batchRelease
 //     static native java.nio.ByteBuffer[] batchRowsWithPartition(long batch, java.nio.ByteBuffer partRow, int partRowBytes,
 //                                                                int numPartFields, boolean[] partVar);   // + a file's partition values
+//     static native void batchRowsAsync(long batch);   // enqueue batchRows' rows and their copy behind the batch's kernels, no wait
+//     static native void batchRowsWithPartitionAsync(long batch, java.nio.ByteBuffer partRow, int partRowBytes, int numPartFields,
+//                                                    boolean[] partVar);
 //     static native long encoderCreate(long schema, int device);
 //     static native void encoderDestroy(long encoder);    // OutputWriter.close (M/TFRecordOutputWriter.scala:40-43)
 //     static native java.nio.ByteBuffer encode(long encoder, long[] columnStructAddrs, int n);   // framed bytes, pinned
@@ -199,6 +202,25 @@ extern "C" JNIEXPORT jobjectArray JNICALL Java_com_linkedin_spark_datasources_tf
   env->SetObjectArrayElement(out, 0, env->NewDirectByteBuffer(const_cast<void*>(rows), (jlong)nb));
   env->SetObjectArrayElement(out, 1, env->NewDirectByteBuffer(const_cast<int64_t*>(offs), (jlong)((n + 1) * 8)));
   return out;
+}
+// The pipelined reader (INTEGRATION.md, submitNext): the rows batchRows / batchRowsWithPartition will return, and their pinned
+// copy, enqueued right after the submit.  The batch stays usable after a failure (batchRows throws the same error again).
+extern "C" JNIEXPORT void JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_batchRowsAsync(JNIEnv* env, jclass, jlong batch) {
+  int32_t rc = tfr_batch_rows_async((tfr_batch*)batch, 1, nullptr, 0, 0, nullptr);
+  if (rc) throw_for(env, rc, -1);
+}
+extern "C" JNIEXPORT void JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_batchRowsWithPartitionAsync(
+    JNIEnv* env, jclass, jlong batch, jobject partRow, jint partRowBytes, jint numPartFields, jbooleanArray partVar) {
+  const void* pr = partRow ? env->GetDirectBufferAddress(partRow) : nullptr;
+  std::vector<uint8_t> var;
+  if (partVar) {
+    jboolean* v = env->GetBooleanArrayElements(partVar, nullptr);
+    var.assign(v, v + env->GetArrayLength(partVar));
+    env->ReleaseBooleanArrayElements(partVar, v, JNI_ABORT);
+  }
+  if ((partVar && (jint)var.size() != numPartFields) || partRowBytes < 0) { throw_for(env, TFR_E_INVALID_ARG, -1); return; }
+  int32_t rc = tfr_batch_rows_async((tfr_batch*)batch, 1, pr, (size_t)partRowBytes, numPartFields, partVar ? var.data() : nullptr);
+  if (rc) throw_for(env, rc, -1);
 }
 extern "C" JNIEXPORT void JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_batchRelease(JNIEnv*, jclass, jlong batch) { if (batch) tfr_batch_release((tfr_batch*)batch); }
 extern "C" JNIEXPORT void JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_encoderDestroy(JNIEnv*, jclass, jlong enc) { if (enc) tfr_encoder_destroy((tfr_encoder*)enc); }
