@@ -343,6 +343,7 @@ static cudaError_t raise_dyn_smem(size_t smem) {
 }
 
 #include "api_decode.inc"
+#include "api_rows.inc"
 
 // ---------------------------------------------------------------------------------------------
 // Arrow C Data Interface export (arrow/c/abi.h structs restated in host_util.h)

@@ -1,5 +1,5 @@
 // host_util.h -- host-side helpers for api.cu: the owners of every CUDA resource a handle holds (device buffers, pinned host
-// buffers, streams, events, the block pools), and the Arrow C Data / Device Interface structs (restated from the Arrow ABI
+// buffers, streams, events, the block pools and the blocks borrowed from them), and the Arrow C Data / Device Interface structs (restated from the Arrow ABI
 // specification, identical in layout to arrow/c/abi.h).
 //
 // This file is the only place that calls the raw allocate / free / create / destroy functions of the CUDA runtime.  Each
@@ -9,6 +9,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <memory>
 #include <utility>
 #include <vector>
 
@@ -95,6 +96,21 @@ class EventPool {
   void give(cudaEvent_t e) { if (e) free_.push_back(e); }
 };
 
+// A block borrowed from a PinnedPool or a DevPool (`bytes` of it asked for) is held by a PoolBlock, empty when the pool could
+// not provide one.  Its destructor and reset() give it back through this deleter, a device block on `st`, the stream whose
+// queued work may still touch it; nothing else does.  The pool must outlive it, and whoever resets it holds the pool's lock.
+template <class Pool>
+struct PoolGiver {
+  Pool* pool = nullptr;
+  cudaStream_t st = nullptr;
+  size_t bytes = 0;
+  void operator()(void* p) const { pool->give_back(p, st); }
+};
+template <class Pool>
+using PoolBlock = std::unique_ptr<void, PoolGiver<Pool>>;
+template <class Pool>
+size_t block_bytes(const PoolBlock<Pool>& b) { return b ? b.get_deleter().bytes : 0; }
+
 struct PinnedPool {
   struct Block { void* p; size_t cap; bool used; };
   std::vector<Block> blocks;
@@ -102,22 +118,24 @@ struct PinnedPool {
   PinnedPool(const PinnedPool&) = delete;
   PinnedPool& operator=(const PinnedPool&) = delete;
   ~PinnedPool() { for (auto& b : blocks) cudaFreeHost(b.p); }
-  void* acquire(size_t bytes) {
+  PoolBlock<PinnedPool> acquire(size_t bytes) {
     int best = -1;
     for (size_t i = 0; i < blocks.size(); ++i)
       if (!blocks[i].used && blocks[i].cap >= bytes && (best < 0 || blocks[i].cap < blocks[best].cap)) best = (int)i;
-    if (best >= 0) { blocks[best].used = true; return blocks[best].p; }
+    if (best >= 0) { blocks[best].used = true; return PoolBlock<PinnedPool>(blocks[best].p, {this, nullptr, bytes}); }
     // drop free blocks that are too small so the pool does not grow without bound
     for (size_t i = 0; i < blocks.size();) {
       if (!blocks[i].used) { cudaFreeHost(blocks[i].p); blocks.erase(blocks.begin() + i); } else ++i;
     }
     void* p = nullptr;
     size_t cap = bytes + bytes / 8 + 4096;
-    if (cudaHostAlloc(&p, cap, cudaHostAllocDefault) != cudaSuccess) return nullptr;
+    if (cudaHostAlloc(&p, cap, cudaHostAllocDefault) != cudaSuccess) return {};
     blocks.push_back({p, cap, true});
-    return p;
+    return PoolBlock<PinnedPool>(p, {this, nullptr, bytes});
   }
-  void give_back(void* p) { for (auto& b : blocks) if (b.p == p) b.used = false; }
+ private:
+  friend struct PoolGiver<PinnedPool>;
+  void give_back(void* p, cudaStream_t) { for (auto& b : blocks) if (b.p == p) b.used = false; }
 };
 
 // device blocks reused across batches.  A block goes back to the pool when its batch is released, possibly while kernels that
@@ -132,7 +150,8 @@ struct DevPool {
   DevPool(const DevPool&) = delete;
   DevPool& operator=(const DevPool&) = delete;
   ~DevPool() { for (auto& b : blocks) { cudaFree(b.p); if (b.ready) cudaEventDestroy(b.ready); } }
-  void* acquire(size_t bytes, cudaEvent_t* ready_out = nullptr) {
+  // `st`: the stream the block goes back on (give_back)
+  PoolBlock<DevPool> acquire(size_t bytes, cudaStream_t st, cudaEvent_t* ready_out = nullptr) {
     int best = -1;
     for (size_t i = 0; i < blocks.size(); ++i) {
       const Block& b = blocks[i];
@@ -143,19 +162,21 @@ struct DevPool {
       const bool same_class = b.cap <= c.cap + c.cap / 8 && c.cap <= b.cap + b.cap / 8;
       if (same_class ? b.stamp < c.stamp : b.cap < c.cap) best = (int)i;
     }
-    if (best >= 0) { blocks[best].used = true; if (ready_out) *ready_out = blocks[best].stamp ? blocks[best].ready : nullptr; return blocks[best].p; }
+    if (best >= 0) { blocks[best].used = true; if (ready_out) *ready_out = blocks[best].stamp ? blocks[best].ready : nullptr; return PoolBlock<DevPool>(blocks[best].p, {this, st, bytes}); }
     for (size_t i = 0; i < blocks.size();) {
       if (!blocks[i].used && blocks.size() > 8) { cudaFree(blocks[i].p); if (blocks[i].ready) cudaEventDestroy(blocks[i].ready); blocks.erase(blocks.begin() + i); } else ++i;
     }
     void* p = nullptr;
     size_t cap = bytes + bytes / 8 + 4096;
-    if (cudaMalloc(&p, cap) != cudaSuccess) { cap = bytes; if (cudaMalloc(&p, cap) != cudaSuccess) return nullptr; }
+    if (cudaMalloc(&p, cap) != cudaSuccess) { cap = bytes; if (cudaMalloc(&p, cap) != cudaSuccess) return {}; }
     blocks.push_back({p, cap, true, nullptr, 0});
     if (ready_out) *ready_out = nullptr;
-    return p;
+    return PoolBlock<DevPool>(p, {this, st, bytes});
   }
+ private:
+  friend struct PoolGiver<DevPool>;
   // `st`: the stream whose queued work may still touch the block
-  void give_back(void* p, cudaStream_t st = nullptr) {
+  void give_back(void* p, cudaStream_t st) {
     for (auto& b : blocks)
       if (b.p == p) {
         b.used = false;

@@ -104,7 +104,9 @@ def test_cuda_resources_are_allocated_and_freed_only_by_their_owners():
     """Every device buffer, pinned host buffer, stream and event of a handle is held by an owner type of host_util.h whose
     destructor frees it, so a create function that returns early frees whatever it had built.  Outside host_util.h nothing
     allocates, frees, creates or destroys one by hand.  The one exception is the device copy of the CRC tables in get_ctx:
-    it lives as long as the process, in static storage, where a destructor would run after the CUDA runtime has shut down."""
+    it lives as long as the process, in static storage, where a destructor would run after the CUDA runtime has shut down.
+    A block borrowed from DevPool or PinnedPool is held the same way, by a PoolBlock that gives it back when it is reset or
+    destroyed: nothing outside host_util.h calls a pool's give_back, so no path can return a block twice or forget one."""
     raw = re.compile(r"\b(cuda(?:Malloc|Free|HostAlloc|StreamCreate|StreamDestroy|EventCreate|EventDestroy)\w*)\s*\(")
     api = dict(_sources())["api.cu"]
     start, body = _braced_body(api, r"static\s+int32_t\s+get_ctx\s*\([^)]*\)\s*\{")
@@ -118,5 +120,6 @@ def test_cuda_resources_are_allocated_and_freed_only_by_their_owners():
                 allowed.append(where)
             else:
                 bad.append(where)
-    assert not bad, "raw CUDA allocations / frees outside the owners of host_util.h:\n" + "\n".join(bad)
+        bad += [f"{f}:{ln}: give_back(" for ln, _ in _calls(code, "give_back")]
+    assert not bad, "raw CUDA allocations / frees, or pool blocks given back, outside the owners of host_util.h:\n" + "\n".join(bad)
     assert len(allowed) == 1, f"get_ctx allocates the CRC tables once: {allowed}"
