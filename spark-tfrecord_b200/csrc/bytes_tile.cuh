@@ -11,6 +11,7 @@
 // tiles fit an SM and grows only when large records leave room for few); XW warps meanwhile copy the payloads out, one
 // record per warp at a time, 4 bytes per lane (conflict-free in shared memory, 128-byte coalesced in global memory).
 #pragma once
+#include "encode.cuh"
 #include "tile.cuh"
 
 // Register bound: 48 resident warps per SM (four 8 + 4 warp tiles, eight 4 + 2 warp tiles), i.e. 40 registers, 16-20 B of
@@ -183,7 +184,7 @@ struct EncBytesArgs {
   const uint8_t* consts;        // g5 | xp16 | zeroed accumulators (bytes_const_bytes())
   uint8_t* out;
   unsigned long long out_cap;
-  uint32_t* small;              // [1] overflow / inconsistent offsets, [2..3] total output bytes
+  EncStatus* st;                // overflow (a payload larger than the slot, inconsistent offsets), total_lo / total_hi
 };
 
 __global__ void bytes_max_len_kernel(const int32_t* __restrict__ offs, uint32_t n_rows, uint32_t* __restrict__ out) {
@@ -227,7 +228,7 @@ __global__ void BYTES_BOUNDS(CW, XW) encode_bytes_kernel(EncBytesArgs A, const u
   const unsigned long long o = (unsigned long long)(lo - off0) + 16ull * row;      // where the framed record starts
   const bool bad = active && (cbytes + 48u > A.slot || lo + len > A.n_values || lo < off0 || o + 16ull + len > A.out_cap);
   if (__any_sync(FULLMASK, bad)) {                          // a payload larger than the slot or inconsistent offsets: the host falls back (every warp sees the same rows: uniform exit)
-    if (threadIdx.x == 0) atomicOr(A.small + 1, 1u);
+    if (threadIdx.x == 0) atomicOr(&A.st->overflow, 1u);
     return;
   }
   if (wid == 0) {
@@ -259,7 +260,7 @@ __global__ void BYTES_BOUNDS(CW, XW) encode_bytes_kernel(EncBytesArgs A, const u
   asm volatile("mov.u32 %0, %1;" : "=r"(T.s) : "r"(smem_u32(tile_b)) : "memory");   // ordered after mbar_wait
   if (row0 + rows == A.n_rows && threadIdx.x == rows - 1) {
     const unsigned long long total = o + 16ull + len;
-    A.small[2] = (uint32_t)total; A.small[3] = (uint32_t)(total >> 32);
+    A.st->total_lo = (uint32_t)total; A.st->total_hi = (uint32_t)(total >> 32);
   }
 
   if (wid < CW) {

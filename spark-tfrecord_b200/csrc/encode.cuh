@@ -21,6 +21,29 @@ struct EncCol {                 // one input column (device pointers)
   const void* values;
 };
 
+// The encoder's status block: one per set of encode buffers on the device, mirrored in pinned host memory.  The size
+// kernels, the row kernels (rows.cuh), encode_bytes_kernel and encode_verdict_kernel report through it, and the host
+// reads a batch's errors, total and launch figures from the mirror.  0xffffffff in a "first row" word: no such row.
+struct EncStatus {
+  uint32_t first_null_row;      // atomicMin: first row with a null in a non-nullable column
+  uint32_t overflow;            // the record-size scan passed 32 bits, or encode_bytes_kernel met a payload or offsets it cannot place
+  uint32_t total_lo, total_hi;  // encode_bytes_kernel: the batch's framed bytes
+  uint32_t max_word;            // atomicMax: largest framed record (Example, SequenceExample) or longest payload (ByteArray)
+  uint32_t pad0[3];
+  uint32_t rows_first_bad;      // row kernels, atomicMin: first malformed row
+  uint32_t rows_first_null;     // row kernels, atomicMin: first row with a null element
+  uint32_t rows_overflow;       // row kernels: a scan of counts overflowed or an arena is too small
+  uint32_t pad1[5];
+  uint32_t verdict_flag;        // encode_verdict_kernel: EVF_* (0: the batch can be emitted as launched)
+  uint32_t verdict_total_lo, verdict_total_hi;   // and the batch's framed bytes
+  uint32_t pad2[13];
+  uint64_t total() const { return total_lo | (uint64_t)total_hi << 32; }
+  uint64_t verdict_total() const { return verdict_total_lo | (uint64_t)verdict_total_hi << 32; }
+};
+static_assert(sizeof(EncStatus) == 128, "the status block is copied whole");
+static_assert(offsetof(EncStatus, total_lo) % 8 == 0, "the host copies a 64-bit scan total onto total_lo / total_hi");
+static_assert(offsetof(EncStatus, rows_overflow) == offsetof(EncStatus, rows_first_bad) + 8, "the row kernels' words are set and copied as a group");
+
 struct EncodeArgs {
   DevSchema sch;
   const EncCol* cols;           // [n_fields]
@@ -28,7 +51,7 @@ struct EncodeArgs {
   const CrcTables* tabs;
   uint32_t* rec_size;           // [n_rows] framed size of each record
   uint32_t* cell_size;          // [n_fields][n_rows] size of the map-entry VALUE (Feature / FeatureList bytes)
-  uint32_t* first_null_err;     // atomicMin: first row with a null in a non-nullable column
+  EncStatus* st;                // (sizes) first_null_row, max_word
   const int32_t* rec_off;       // [n_rows+1] (emit)
   uint8_t* out;                 // (emit)
 };
@@ -238,8 +261,8 @@ __global__ void __launch_bounds__(256) encode_kernel(EncodeArgs A, const uint32_
     }
     uint32_t plen = 1 + vsize32(gsize[0]) + gsize[0] + (seq ? 1 + vsize32(gsize[1]) + gsize[1] : 0);
     if (MODE == 0) {
-      if (__any_sync(FULLMASK, null_err) && lane == 0) atomicMin(A.first_null_err, row);
-      if (lane == 0) { A.rec_size[row] = 16 + plen; atomicMax(A.first_null_err + 4, 16 + plen); }   // [4]: largest framed record (encode_tile.cuh slot)
+      if (__any_sync(FULLMASK, null_err) && lane == 0) atomicMin(&A.st->first_null_row, row);
+      if (lane == 0) { A.rec_size[row] = 16 + plen; atomicMax(&A.st->max_word, 16 + plen); }
       continue;
     }
     uint8_t* rec = A.out + A.rec_off[row];
@@ -262,13 +285,12 @@ __global__ void __launch_bounds__(256) encode_kernel(EncodeArgs A, const uint32_
 // ---------------------------------------------------------------------------------------------
 // Verdict of a pipelined encode (api_encode.inc, tfr_encode_rows_submit).  Its outputs were sized from what the encoder
 // learned on earlier batches, not from this batch's sizes; one thread checks them after the record-size scan and raises
-// v[EV_FLAG] when the batch cannot be emitted as launched.  The guarded emit kernels read that word first, so a flagged batch
-// writes nothing; the host redoes it through the synchronous path.  The total and the first error rows go to the verdict too.
+// EncStatus::verdict_flag when the batch cannot be emitted as launched.  The guarded emit kernels read that word first, so
+// a flagged batch writes nothing; the host redoes it through the synchronous path.  The total goes to the verdict too.
 // ---------------------------------------------------------------------------------------------
-enum { EV_FLAG = 16, EV_TOTAL_LO = 17, EV_TOTAL_HI = 18 };     // words of the encoder's small block, behind the ones of encode.cuh / rows.cuh
 enum { EVF_CAPACITY = 1, EVF_SLOT = 2, EVF_STRIDE = 4, EVF_ROWS = 8, EVF_NULL = 16 };
 struct EncVerdictArgs {
-  uint32_t* small;                       // [0] first null row, [1] scan overflow, [4] largest framed record / payload, [8..10] row path
+  EncStatus* st;
   const unsigned long long* total;       // Example / SequenceExample: the scan's grand total
   const int32_t* bytes_offs;             // ByteArray: the column's offsets (total = offs[n] - offs[0] + 16 n); null otherwise
   uint32_t n_rows;
@@ -278,21 +300,21 @@ struct EncVerdictArgs {
 };
 __global__ void encode_verdict_kernel(EncVerdictArgs A) {
   if (threadIdx.x | blockIdx.x) return;
-  uint32_t* s = A.small;
+  EncStatus* s = A.st;
   uint32_t flag = 0;
   unsigned long long total;
   if (A.bytes_offs) {
     const int32_t o0 = A.bytes_offs[0], on = A.bytes_offs[A.n_rows];
     total = on >= o0 && o0 >= 0 ? (unsigned long long)(on - o0) + 16ull * A.n_rows : ~0ull;
-    if (s[4] > A.max_len) flag |= EVF_STRIDE;
+    if (s->max_word > A.max_len) flag |= EVF_STRIDE;
   } else {
     total = *A.total;
-    if (s[1]) flag |= EVF_CAPACITY;
-    if (A.max_rec && s[4] > A.max_rec) flag |= EVF_SLOT;
+    if (s->overflow) flag |= EVF_CAPACITY;
+    if (A.max_rec && s->max_word > A.max_rec) flag |= EVF_SLOT;
   }
   if (total > A.cap || total > 0x7fffffffull) flag |= EVF_CAPACITY;
-  if (s[8] != 0xffffffffu || s[9] != 0xffffffffu || s[10]) flag |= EVF_ROWS;
-  if (s[0] != 0xffffffffu) flag |= EVF_NULL;
-  s[EV_FLAG] = flag;
-  s[EV_TOTAL_LO] = (uint32_t)total; s[EV_TOTAL_HI] = (uint32_t)(total >> 32);
+  if (s->rows_first_bad != 0xffffffffu || s->rows_first_null != 0xffffffffu || s->rows_overflow) flag |= EVF_ROWS;
+  if (s->first_null_row != 0xffffffffu) flag |= EVF_NULL;
+  s->verdict_flag = flag;
+  s->verdict_total_lo = (uint32_t)total; s->verdict_total_hi = (uint32_t)(total >> 32);
 }

@@ -60,7 +60,7 @@ struct EncSizeArgs {
   uint32_t n_rows;
   uint32_t* rec_size;           // [n_rows]
   uint32_t* cell_size;          // [n_fields][n_rows]
-  uint32_t* small;              // [0] atomicMin first row with a null in a non-nullable column, [4] atomicMax framed record size
+  EncStatus* st;                // first_null_row, max_word
 };
 __global__ void __launch_bounds__(ENC_SIZE_THREADS, 6) encode_tile_size_kernel(EncSizeArgs A) {
   __shared__ uint32_t sacc[ENC_TILE_ROWS];
@@ -92,13 +92,13 @@ __global__ void __launch_bounds__(ENC_SIZE_THREADS, 6) encode_tile_size_kernel(E
       else sum += entry_total(fd, V);
     }
   if (sum) atomicAdd(&sacc[lane], sum);
-  if (null_err) atomicMin(A.small, row);
+  if (null_err) atomicMin(&A.st->first_null_row, row);
   __syncthreads();
   if (wid == 0 && active) {
     const uint32_t G = sacc[lane], sz = 16 + 1 + vsize32(G) + G;
     A.rec_size[row] = sz;
     const uint32_t mx = __reduce_max_sync(__activemask(), sz);
-    if (lane == 0) atomicMax(A.small + 4, mx);
+    if (lane == 0) atomicMax(&A.st->max_word, mx);
   }
 }
 

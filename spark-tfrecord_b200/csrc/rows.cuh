@@ -39,7 +39,7 @@ struct RowsArgs {
   int32_t* const* lev;          // [n_cnt] scan outputs: level 0 = the column's Arrow offsets, levels 1, 2 = per-row bases
   EncCol* cols;                 // [n_fields] the encoder's columns; the layout kernel fills the inner offsets and values
   uint32_t smem_cap;            // tile bytes the shared-memory staging holds
-  uint32_t* small;              // [8] first malformed row, [9] first row with a null element, [10] overflow
+  EncStatus* st;                // rows_first_bad, rows_first_null, rows_overflow
 };
 
 enum { RW_OK = 0, RW_NULL = 1, RW_BAD = 2 };
@@ -182,8 +182,8 @@ __global__ void __launch_bounds__(ROWS_TILE) rows_pass_a_kernel(RowsArgs A) {
     if (room > len) bad = true;
   }
   const uint32_t mb = __ballot_sync(FULLMASK, bad), mn = __ballot_sync(FULLMASK, nul && !bad);
-  if (mb && lane == (uint32_t)__ffs(mb) - 1) atomicMin(A.small + 8, r);
-  if (mn && lane == (uint32_t)__ffs(mn) - 1) atomicMin(A.small + 9, r);
+  if (mb && lane == (uint32_t)__ffs(mb) - 1) atomicMin(&A.st->rows_first_bad, r);
+  if (mn && lane == (uint32_t)__ffs(mn) - 1) atomicMin(&A.st->rows_first_null, r);
   const bool ok = active && !bad && !nul;
 
   // ---- columns ----
@@ -228,7 +228,7 @@ __global__ void rows_layout_kernel(RowsArgs A, const unsigned long long* __restr
       for (int l = 1; l < fd.n_levels; ++l) ipos += totals[fd.cnt_slot + l - 1] + 1;
       vpos = ((vpos + 15) & ~15ull) + totals[fd.cnt_slot + fd.n_levels - 1] * (unsigned long long)fd.width;
     }
-    over = (A.small[10] != 0 || vpos > vcap || ipos > icap) ? 1u : 0u;
+    over = (A.st->rows_overflow != 0 || vpos > vcap || ipos > icap) ? 1u : 0u;
     if (!over && blockIdx.x == 0) {
       vpos = ipos = 0;
       for (uint32_t f = 0; f < nf; ++f) {
@@ -246,7 +246,7 @@ __global__ void rows_layout_kernel(RowsArgs A, const unsigned long long* __restr
         vpos += totals[fd.cnt_slot + fd.n_levels - 1] * (unsigned long long)fd.width;
       }
     }
-    if (over && blockIdx.x == 0) A.small[10] = 1;
+    if (over && blockIdx.x == 0) A.st->rows_overflow = 1;
   }
   __syncthreads();
   if (!over) return;
@@ -301,7 +301,7 @@ __device__ __forceinline__ void rows_copy_elems(const DevField& fd, void* values
 }
 
 __global__ void __launch_bounds__(ROWS_B_WARPS * 32) rows_pass_b_kernel(RowsArgs A) {
-  if (A.small[10]) return;                                   // the columns were not placed: nothing to fill
+  if (A.st->rows_overflow) return;                                   // the columns were not placed: nothing to fill
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t w = blockIdx.x * ROWS_B_WARPS + (threadIdx.x >> 5);
   const uint32_t r = w * 32 + lane;
