@@ -420,7 +420,7 @@ extern "C" int32_t tfr_batch_export_arrow_host(tfr_batch* b, int32_t column, voi
   if (!b || !arrow_array || !arrow_schema || column < 0 || column >= (int32_t)b->cols.size()) return fail(TFR_E_INVALID_ARG, "bad argument");
   int32_t rc = tfr_batch_to_host(b, nullptr, (int32_t)b->cols.size());
   if (rc) return rc;
-  const tfr_column& c = b->host_cols[column];
+  const tfr_column& c = b->host_copy.cols[column];
   const tfr_schema& S = b->dec->schema;
   std::string nm((const char*)&S.names[S.fields[column].name_off], S.fields[column].name_len);
   build_schema((ArrowSchema*)arrow_schema, nm.c_str(), c.elem_type, c.depth);

@@ -1,5 +1,5 @@
 // host_util.h -- host-side helpers for api.cu: the owners of every CUDA resource a handle holds (device buffers, pinned host
-// buffers, streams, events, the block pools and the blocks borrowed from them), and the Arrow C Data / Device Interface structs (restated from the Arrow ABI
+// buffers, streams, events, the block and event pools and what is borrowed from them), and the Arrow C Data / Device Interface structs (restated from the Arrow ABI
 // specification, identical in layout to arrow/c/abi.h).
 //
 // This file is the only place that calls the raw allocate / free / create / destroy functions of the CUDA runtime.  Each
@@ -76,25 +76,42 @@ class Event {
   operator cudaEvent_t() const { return e_; }
 };
 
+// An event borrowed from an EventPool is held by a PoolEvent, null until taken.  Like a PoolBlock, its destructor and
+// reset() give it back through this deleter, and nothing else does.  The pool must outlive it, and whoever resets it holds
+// the pool's lock.
+class EventPool;
+struct EventGiver {
+  EventPool* pool = nullptr;
+  inline void operator()(cudaEvent_t e) const;
+};
+using PoolEvent = std::unique_ptr<CUevent_st, EventGiver>;
+
 // Events lent out and taken back (a batch's completion, a profiling span's ends).  The pool owns every event it ever
-// created; borrowers hold plain handles and never destroy them.
+// created; borrowers hold them in PoolEvents and never destroy them.
 class EventPool {
   unsigned flags_;
   std::vector<cudaEvent_t> all_, free_;
+  friend struct EventGiver;
+  void give(cudaEvent_t e) { free_.push_back(e); }
  public:
   explicit EventPool(unsigned flags) : flags_(flags) {}
   EventPool(const EventPool&) = delete;
   EventPool& operator=(const EventPool&) = delete;
   ~EventPool() { for (cudaEvent_t e : all_) cudaEventDestroy(e); }
-  cudaError_t take(cudaEvent_t* out) {
-    if (!free_.empty()) { *out = free_.back(); free_.pop_back(); return cudaSuccess; }
+  // `out` is empty; it stays empty when no event can be created
+  cudaError_t take(PoolEvent& out) {
     cudaEvent_t e = nullptr;
-    cudaError_t err = cudaEventCreateWithFlags(&e, flags_);
-    if (err == cudaSuccess) { all_.push_back(e); *out = e; }
-    return err;
+    if (!free_.empty()) { e = free_.back(); free_.pop_back(); }
+    else {
+      const cudaError_t err = cudaEventCreateWithFlags(&e, flags_);
+      if (err != cudaSuccess) return err;
+      all_.push_back(e);
+    }
+    out = PoolEvent(e, EventGiver{this});
+    return cudaSuccess;
   }
-  void give(cudaEvent_t e) { if (e) free_.push_back(e); }
 };
+inline void EventGiver::operator()(cudaEvent_t e) const { pool->give(e); }
 
 // A block borrowed from a PinnedPool or a DevPool (`bytes` of it asked for) is held by a PoolBlock, empty when the pool could
 // not provide one.  Its destructor and reset() give it back through this deleter, a device block on `st`, the stream whose

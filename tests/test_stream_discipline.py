@@ -106,7 +106,8 @@ def test_cuda_resources_are_allocated_and_freed_only_by_their_owners():
     allocates, frees, creates or destroys one by hand.  The one exception is the device copy of the CRC tables in get_ctx:
     it lives as long as the process, in static storage, where a destructor would run after the CUDA runtime has shut down.
     A block borrowed from DevPool or PinnedPool is held the same way, by a PoolBlock that gives it back when it is reset or
-    destroyed: nothing outside host_util.h calls a pool's give_back, so no path can return a block twice or forget one."""
+    destroyed: nothing outside host_util.h calls a pool's give_back, so no path can return a block twice or forget one.  An
+    event borrowed from an EventPool is held by a PoolEvent in the same way: nothing outside host_util.h calls a pool's give."""
     raw = re.compile(r"\b(cuda(?:Malloc|Free|HostAlloc|StreamCreate|StreamDestroy|EventCreate|EventDestroy)\w*)\s*\(")
     api = dict(_sources())["api.cu"]
     start, body = _braced_body(api, r"static\s+int32_t\s+get_ctx\s*\([^)]*\)\s*\{")
@@ -120,6 +121,6 @@ def test_cuda_resources_are_allocated_and_freed_only_by_their_owners():
                 allowed.append(where)
             else:
                 bad.append(where)
-        bad += [f"{f}:{ln}: give_back(" for ln, _ in _calls(code, "give_back")]
-    assert not bad, "raw CUDA allocations / frees, or pool blocks given back, outside the owners of host_util.h:\n" + "\n".join(bad)
+        bad += [f"{f}:{ln}: {name}(" for name in ("give_back", "give") for ln, _ in _calls(code, name)]
+    assert not bad, "raw CUDA allocations / frees, or pool blocks or events given back, outside the owners of host_util.h:\n" + "\n".join(bad)
     assert len(allowed) == 1, f"get_ctx allocates the CRC tables once: {allowed}"
