@@ -101,6 +101,17 @@ int32_t tfr_schema_num_fields(const tfr_schema*);
 /* ---- decode: replaces the body of the buildReader closure ---------------------------- */
 /* flags */
 #define TFR_F_VERIFY_CRC   0x1u  /* tensorflow-hadoop's CRC check (on by default there)   */
+/* Spark's mode=DROPMALFORMED: a record that fails is dropped and decoding goes on (the default, FAILFAST, stops the block
+ * at it).  Record errors are TFR_E_CRC_DATA, TFR_E_MALFORMED_PROTO, TFR_E_KIND_MISMATCH, TFR_E_EMPTY_SCALAR,
+ * TFR_E_NULL_IN_NONNULL and TFR_E_BAD_NESTING: a dropped record's length CRC verified, so the next frame is known.  The
+ * batch's rows, columns, null counts and UnsafeRows are those of the block with the dropped frames cut out.  Framing errors
+ * (TFR_E_CRC_LENGTH, TFR_E_TRUNCATED, TFR_E_RECORD_TOO_LARGE) still end the block, as without the flag: the frame chain is
+ * lost there.  tfr_batch_info in drop mode: n_rows = the rows delivered; n_records = the frames in the consumed bytes,
+ * dropped ones included; consumed_bytes = what tfr_batch_consumed returns; error_code / error_row / error_field are set
+ * for a framing error only, and error_row is then the frame index at which framing stopped, which can exceed n_rows by the
+ * records dropped before it.  tfr_batch_dropped lists the dropped records.  Without TFR_F_VERIFY_CRC no CRC is checked,
+ * so nothing is dropped for one.                                                                                          */
+#define TFR_F_DROP_MALFORMED 0x2u
 #define TFR_F_DEFAULT      (TFR_F_VERIFY_CRC)
 
 /* Replaces TFRecordFileReader.readFile's setup (M/TFRecordFileReader.scala:16-44):
@@ -167,7 +178,7 @@ int32_t tfr_decoder_get_profile(tfr_decoder*, double* ms /* [TFR_PROFILE_STAGES]
  * [5] column shapes (re)learned, [6] batches re-run by the single-pass kernel's transcoding instantiation (malformed
  * UTF-8 in a string column), [7] rows passes enqueued by tfr_batch_rows_async without a host synchronisation, [8] of
  * those rebuilt through the synchronous rows path (the batch was redone, or the rows did not fit what they were
- * launched with).  A caller passing n = 8 gets the first eight.                                                   */
+ * launched with), [9] records dropped (TFR_F_DROP_MALFORMED).  A caller passing n = 8 gets the first eight.        */
 int32_t tfr_decoder_get_stats(tfr_decoder*, int64_t* out, int32_t n /* <= 10 */);
 
 int32_t tfr_batch_wait(tfr_batch*);
@@ -189,6 +200,13 @@ int32_t tfr_batch_status(tfr_batch*, tfr_batch_info* out);
  * index of block t+1.  For a batch that later reports an error, tfr_batch_info.consumed_bytes (the bytes in front of the
  * failing record) is what counts; the reader stops there anyway.                                                     */
 int32_t tfr_batch_consumed(tfr_batch*, size_t* consumed);
+/* The records a TFR_F_DROP_MALFORMED decoder dropped from this batch.  Waits for and resolves the batch like
+ * tfr_batch_status, sets *n_dropped to their number and fills the first min(*n_dropped, cap) entries, in record order:
+ * the frame index within the block, the frame's byte offset in the submitted buffer (a reader adds the block's file
+ * offset to log where the record was), the TFR_E_* code and the schema field (-1 when none).  Any of the arrays may be
+ * NULL, and all of them when cap = 0.  Without the flag *n_dropped is 0.                                               */
+int32_t tfr_batch_dropped(tfr_batch*, int64_t* n_dropped, int64_t* record, int64_t* offset, int32_t* code, int32_t* field,
+                          int64_t cap);
 
 /* One output column in Arrow layout.  n_levels offset arrays (int32, Arrow list/binary
  * offsets) from the outermost (one entry per row + 1) to the innermost, then the leaf

@@ -29,7 +29,12 @@ TFR_E_NULL_IN_NONNULL = -17
 TFR_E_BAD_NESTING = -18
 
 TFR_F_VERIFY_CRC = 0x1
+TFR_F_DROP_MALFORMED = 0x2       # mode=DROPMALFORMED: failing records are dropped, framing errors still end the block
 TFR_F_DEFAULT = TFR_F_VERIFY_CRC
+
+# the record errors a TFR_F_DROP_MALFORMED decoder drops (the other data errors are framing errors)
+RECORD_ERRORS = (TFR_E_CRC_DATA, TFR_E_MALFORMED_PROTO, TFR_E_KIND_MISMATCH, TFR_E_EMPTY_SCALAR, TFR_E_NULL_IN_NONNULL,
+                 TFR_E_BAD_NESTING)
 
 STATUS_NAMES = {v: k for k, v in list(globals().items()) if k.startswith("TFR_E_") or k == "TFR_OK"}
 

@@ -17,6 +17,7 @@
 
 #include "common.cuh"
 #include "decode.cuh"
+#include "drop.cuh"
 #include "encode.cuh"
 #include "encode_tile.cuh"
 #include "bytes_tile.cuh"

@@ -20,17 +20,19 @@ bytes, list, list of lists) standing in for Catalyst's InternalRow; message argu
 protobuf bytes (there are no org.tensorflow.example classes here)."""
 from __future__ import annotations
 
+import logging
 import os
 import struct
 from typing import Dict, Iterator, List, Optional, Sequence
 
 import numpy as np
 
-from . import _native
-from ._cabi import TFR_F_DEFAULT, TFR_E_BATCH_TOO_LARGE as A_TFR_E_BATCH_TOO_LARGE, columns_from_rows
+from . import _cabi, _native
+from ._cabi import TFR_F_DEFAULT, TFR_F_DROP_MALFORMED, TFR_E_BATCH_TOO_LARGE as A_TFR_E_BATCH_TOO_LARGE, columns_from_rows
 from .sqltypes import RECORD_TYPES, StructType, byte_array_schema
 
 M = "src/main/scala/com/linkedin/spark/datasources/tfrecord/"
+_LOG = logging.getLogger(__name__)
 
 
 def _record_type(options: Optional[Dict[str, str]]) -> int:
@@ -38,6 +40,22 @@ def _record_type(options: Optional[Dict[str, str]]) -> int:
     if rt not in RECORD_TYPES:                                  # :78-79
         raise _native.IllegalArgumentException(-3, f"Unsupported recordType {rt}: recordType can be ByteArray, Example or SequenceExample")
     return RECORD_TYPES[rt]
+
+
+def _decoder_flags(options: Optional[Dict[str, str]]) -> int:
+    """the `mode` option, case-insensitive as Spark's ParseMode reads it -> decoder flags.  FAILFAST (the default, the
+    reference's behaviour): the first failing record ends the file.  DROPMALFORMED: failing records are dropped and the
+    rest is read (framing errors still end the file).  PERMISSIVE needs a corrupt-record column, which this source has not."""
+    mode = (options or {}).get("mode", "FAILFAST")
+    m = mode.upper() if isinstance(mode, str) else mode
+    if m == "FAILFAST":
+        return TFR_F_DEFAULT
+    if m == "DROPMALFORMED":
+        return TFR_F_DEFAULT | TFR_F_DROP_MALFORMED
+    if m == "PERMISSIVE":
+        raise _native.IllegalArgumentException(-1, "mode PERMISSIVE is not supported: the tfrecord source has no corrupt-record "
+                                                   "column; use FAILFAST or DROPMALFORMED")
+    raise _native.IllegalArgumentException(-1, f"mode {mode}: the tfrecord source supports FAILFAST and DROPMALFORMED")
 
 
 # ---- stream compression (SURVEY 8f.3): host-side, around the same GPU kernels -------------------------------------------
@@ -259,10 +277,13 @@ class TFRecordFileReader:
         """Stages the file in blocks into the decoder's pinned staging slots and decodes each block on the GPU
         (tfr_decode_submit); where a block ends -- the carry into the next one -- is known as soon as its frame index has
         run (tfr_batch_consumed), so block k+1 is read and submitted while block k decodes and block k-1's rows are
-        handed out.  Rows before a bad record are yielded, then the exception the reference would throw is raised."""
+        handed out.  Rows before a bad record are yielded, then the exception the reference would throw is raised.
+        With options["mode"] = "DROPMALFORMED" a failing record is skipped instead (a framing error still raises), and
+        the dropped records of each block are logged once, with the file offset of the first."""
         rt = _record_type(options)
+        flags = _decoder_flags(options)
         block = block_bytes or TFRecordFileReader.BLOCK_BYTES
-        dec = _native.Decoder(schema, rt, device, TFR_F_DEFAULT)
+        dec = _native.Decoder(schema, rt, device, flags)
 
         def gen():
             todo = []
@@ -274,6 +295,7 @@ class TFRecordFileReader:
                     remaining = (1 << 62) if compressed else file.length          # a compressed file is read to its end
                     n_slots = dec.num_staging_slots()
                     turn = [0]
+                    pos = [0 if compressed else file.start]     # where the next block starts in the (decompressed) file
 
                     def stage(nbytes):
                         st = dec.staging_slot(turn[0] % n_slots, nbytes)
@@ -282,24 +304,32 @@ class TFRecordFileReader:
 
                     def process(st, nbytes, final):
                         batch = dec.submit(st, is_final=final, nbytes=nbytes)
-                        todo.append(batch)
-                        return batch.consumed()
+                        todo.append((batch, pos[0]))
+                        used = batch.consumed()
+                        pos[0] += used
+                        return used
 
-                    def drain(batch):
+                    def drain(batch, block_pos):
                         try:
                             for row in _rows_of(batch):
                                 yield row
+                            if flags & TFR_F_DROP_MALFORMED:
+                                dropped = batch.dropped()
+                                if dropped:
+                                    _LOG.warning("%s: dropped %d malformed record(s) of the block at offset %d; the first at "
+                                                 "file offset %d (%s)", file.toPath(), len(dropped), block_pos,
+                                                 block_pos + dropped[0][1], _cabi.STATUS_NAMES.get(dropped[0][2], dropped[0][2]))
                             batch.raise_if_error()
                         finally:
                             batch.release()
 
                     for _ in _stream_blocks(f, remaining, block, stage, process):
                         while len(todo) > 1:                 # the block before the one just submitted
-                            yield from drain(todo.pop(0))
+                            yield from drain(*todo.pop(0))
                     while todo:
-                        yield from drain(todo.pop(0))
+                        yield from drain(*todo.pop(0))
             finally:
-                for batch in todo:
+                for batch, _ in todo:
                     batch.release()
                 dec.close()
 
@@ -408,7 +438,9 @@ class DefaultSource:
         return codes_to_struct(allreduce_schema(local, dist, f"cuda:{device}" if dist is not None and dist.is_initialized() and dist.get_backend() == "nccl" else None))
 
     def buildReader(self, dataSchema: StructType, requiredSchema: StructType, options: Dict[str, str], device: int = 0):
-        """-> PartitionedFile => Iterator[row] (filters are accepted and ignored, :123)"""
+        """-> PartitionedFile => Iterator[row] (filters are accepted and ignored, :123).  options["mode"]: FAILFAST (default)
+        or DROPMALFORMED, checked here, before any file is read."""
+        _decoder_flags(options)
         return lambda file: TFRecordFileReader.readFile(None, options, file, requiredSchema, device)
 
     def prepareWrite(self, options: Dict[str, str], dataSchema: StructType):

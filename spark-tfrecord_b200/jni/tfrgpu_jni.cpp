@@ -16,6 +16,7 @@
 //     static native long[] batchStatus(long batch);      // {nRows, nRecords, consumed, errorCode, errorRow, errorField}; waits for a submitted batch
 //     static native java.nio.ByteBuffer[] batchColumnHost(long batch, int column, long[] meta);  // validity, offsets*, values
 //     static native void batchExportArrowDevice(long batch, int column, long arrowDeviceArrayAddr, long arrowSchemaAddr);  // ColumnarBatch on the GPU (spark-rapids)
+//     static native long[] batchDropped(long batch, int maxEntries);   // {nDropped, (record, offset, code, field)*}: DROPMALFORMED
 //     static native void batchThrowIfError(long batch);   // the exception the reference would throw for the first failing record
 //     static native void batchRelease(long batch);
 //     static native java.nio.ByteBuffer[] batchRows(long batch);   // {rows, int64 row offsets}: pinned UnsafeRows, valid until batchRelease
@@ -133,6 +134,23 @@ extern "C" JNIEXPORT jlongArray JNICALL Java_com_linkedin_spark_datasources_tfre
   if (rc0) { tfr_batch_release((tfr_batch*)batch); throw_for(env, rc0, -1); return nullptr; }   // a CUDA failure: the batch is gone, the task fails
   jlong v[6] = {i.n_rows, i.n_records, i.consumed_bytes, i.error_code, i.error_row, i.error_field};
   jlongArray a = env->NewLongArray(6); env->SetLongArrayRegion(a, 0, 6, v);
+  return a;
+}
+// mode=DROPMALFORMED (decoder flag TFR_F_DROP_MALFORMED): {nDropped, then per dropped record up to maxEntries of them
+// record, offset, code, field}.  The reader logs the count and the first record's file offset (block offset + offset) once
+// per block; it waits for a submitted batch like batchStatus.
+extern "C" JNIEXPORT jlongArray JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_batchDropped(JNIEnv* env, jclass, jlong batch, jint maxEntries) {
+  int64_t n = 0;
+  int32_t rc = tfr_batch_dropped((tfr_batch*)batch, &n, nullptr, nullptr, nullptr, nullptr, 0);
+  if (rc) { tfr_batch_release((tfr_batch*)batch); throw_for(env, rc, -1); return nullptr; }
+  const int64_t k = maxEntries < 0 ? 0 : (n < maxEntries ? n : (int64_t)maxEntries);
+  std::vector<int64_t> rec(k), off(k);
+  std::vector<int32_t> code(k), field(k);
+  if (k) tfr_batch_dropped((tfr_batch*)batch, &n, rec.data(), off.data(), code.data(), field.data(), k);
+  std::vector<jlong> v(1 + 4 * k);
+  v[0] = (jlong)n;
+  for (int64_t i = 0; i < k; ++i) { v[1 + 4 * i] = rec[i]; v[2 + 4 * i] = off[i]; v[3 + 4 * i] = code[i]; v[4 + 4 * i] = field[i]; }
+  jlongArray a = env->NewLongArray((jsize)v.size()); env->SetLongArrayRegion(a, 0, (jsize)v.size(), v.data());
   return a;
 }
 // The Scala iterator calls this once per column, wraps the buffers in OnHeap/OffHeap column vectors (or an
