@@ -112,11 +112,29 @@ int32_t tfr_schema_num_fields(const tfr_schema*);
  * records dropped before it.  tfr_batch_dropped lists the dropped records.  Without TFR_F_VERIFY_CRC no CRC is checked,
  * so nothing is dropped for one.                                                                                          */
 #define TFR_F_DROP_MALFORMED 0x2u
+/* Spark's mode=PERMISSIVE: a record that fails with one of the record errors above does not end the block and is not
+ * dropped: it yields one row, at its own position in record order, whose data fields are all null -- non-nullable ones
+ * included, as Spark reads file sources with a nullable data schema.  The row's fixed-width values are 0 and every list or
+ * string column has a zero-length entry there.  With a corrupt-record column (tfr_decoder_create_permissive) that column
+ * holds the record's payload (the bytes between the 12-byte header and the 4-byte data CRC, for a payload-CRC failure
+ * too) on such a row and is null on every other row; a feature of that name in a record is never looked up (it is still
+ * validated, like any feature outside the schema).  Framing errors still end the block.  tfr_batch_info in PERMISSIVE:
+ * n_rows = every frame before the framing stop, failing ones included; n_records and consumed_bytes as without the flag;
+ * error_code / error_row / error_field are set for a framing error only, and error_row then equals n_rows.
+ * tfr_batch_dropped lists the records delivered as corrupt rows (the frame index is the row index).  Example and
+ * SequenceExample only; with TFR_F_DROP_MALFORMED or for TFR_RT_BYTE_ARRAY the create call returns TFR_E_INVALID_ARG.  */
+#define TFR_F_PERMISSIVE   0x4u
 #define TFR_F_DEFAULT      (TFR_F_VERIFY_CRC)
 
 /* Replaces TFRecordFileReader.readFile's setup (M/TFRecordFileReader.scala:16-44):
  * binds a device, a CUDA stream and reusable device/pinned buffers.                        */
 int32_t tfr_decoder_create(const tfr_schema*, int32_t device, uint32_t flags, tfr_decoder** out);
+/* A TFR_F_PERMISSIVE decoder (the flag is required) whose schema field `corrupt_field` is the corrupt-record column:
+ * BinaryType, depth 0 and nullable, or TFR_E_INVALID_ARG naming the field.  corrupt_field = -1: no such column (corrupt
+ * records are rows of nulls only), which is what tfr_decoder_create with TFR_F_PERMISSIVE does.  Argument errors are
+ * returned before any device work.                                                                                     */
+int32_t tfr_decoder_create_permissive(const tfr_schema*, int32_t device, uint32_t flags, int32_t corrupt_field,
+                                      tfr_decoder** out);
 void    tfr_decoder_destroy(tfr_decoder*);
 
 /* Pinned host staging the caller fills with framed file bytes (the JVM sees it as a direct
@@ -178,7 +196,9 @@ int32_t tfr_decoder_get_profile(tfr_decoder*, double* ms /* [TFR_PROFILE_STAGES]
  * [5] column shapes (re)learned, [6] batches re-run by the single-pass kernel's transcoding instantiation (malformed
  * UTF-8 in a string column), [7] rows passes enqueued by tfr_batch_rows_async without a host synchronisation, [8] of
  * those rebuilt through the synchronous rows path (the batch was redone, or the rows did not fit what they were
- * launched with), [9] records dropped (TFR_F_DROP_MALFORMED).  A caller passing n = 8 gets the first eight.        */
+ * launched with), [9] records dropped (TFR_F_DROP_MALFORMED), [10] records delivered as corrupt rows
+ * (TFR_F_PERMISSIVE).  A caller passing n = 8 gets the first eight; n <= 11 gets them all, counter [10] being
+ * PERMISSIVE's, and a caller passing 10 or fewer is unaffected.                                                     */
 int32_t tfr_decoder_get_stats(tfr_decoder*, int64_t* out, int32_t n /* <= 10 */);
 
 int32_t tfr_batch_wait(tfr_batch*);
@@ -204,7 +224,8 @@ int32_t tfr_batch_consumed(tfr_batch*, size_t* consumed);
  * tfr_batch_status, sets *n_dropped to their number and fills the first min(*n_dropped, cap) entries, in record order:
  * the frame index within the block, the frame's byte offset in the submitted buffer (a reader adds the block's file
  * offset to log where the record was), the TFR_E_* code and the schema field (-1 when none).  Any of the arrays may be
- * NULL, and all of them when cap = 0.  Without the flag *n_dropped is 0.                                               */
+ * NULL, and all of them when cap = 0.  Without the flag *n_dropped is 0.  A TFR_F_PERMISSIVE decoder lists the records
+ * it delivered as corrupt rows, in the same format; their frame index is also their row index.                        */
 int32_t tfr_batch_dropped(tfr_batch*, int64_t* n_dropped, int64_t* record, int64_t* offset, int32_t* code, int32_t* field,
                           int64_t cap);
 

@@ -30,6 +30,7 @@ TFR_E_BAD_NESTING = -18
 
 TFR_F_VERIFY_CRC = 0x1
 TFR_F_DROP_MALFORMED = 0x2       # mode=DROPMALFORMED: failing records are dropped, framing errors still end the block
+TFR_F_PERMISSIVE = 0x4           # mode=PERMISSIVE: a failing record is a row of nulls (its payload in the corrupt-record column)
 TFR_F_DEFAULT = TFR_F_VERIFY_CRC
 
 # the record errors a TFR_F_DROP_MALFORMED decoder drops (the other data errors are framing errors)

@@ -21,7 +21,7 @@ _LIB = None
 # every symbol include/tfrgpu.h declares
 EXPORTS = [
     "tfr_abi_version", "tfr_status_string", "tfr_last_error", "tfr_schema_create", "tfr_schema_destroy",
-    "tfr_schema_num_fields", "tfr_decoder_create", "tfr_decoder_destroy", "tfr_decoder_staging", "tfr_decoder_staging_slot",
+    "tfr_schema_num_fields", "tfr_decoder_create", "tfr_decoder_create_permissive", "tfr_decoder_destroy", "tfr_decoder_staging", "tfr_decoder_staging_slot",
     "tfr_decoder_num_staging_slots", "tfr_decode", "tfr_decode_submit",
     "tfr_decoder_stream", "tfr_decoder_set_profiling", "tfr_decoder_get_profile", "tfr_decoder_get_stats", "tfr_batch_wait", "tfr_batch_status", "tfr_batch_consumed", "tfr_batch_dropped", "tfr_batch_num_columns", "tfr_batch_columns",
     "tfr_batch_to_host_async", "tfr_batch_to_host", "tfr_batch_export_arrow_host", "tfr_batch_export_arrow_device", "tfr_batch_release",
@@ -105,6 +105,7 @@ def lib():
         "tfr_schema_destroy": (None, [vp]),
         "tfr_schema_num_fields": (i32, [vp]),
         "tfr_decoder_create": (i32, [vp, i32, u32, P(vp)]),
+        "tfr_decoder_create_permissive": (i32, [vp, i32, u32, i32, P(vp)]),
         "tfr_decoder_destroy": (None, [vp]),
         "tfr_decoder_staging": (i32, [vp, sz, P(vp), P(sz)]),
         "tfr_decoder_staging_slot": (i32, [vp, i32, sz, P(vp), P(sz)]),
@@ -237,7 +238,8 @@ class Batch:
         return n.value
 
     def dropped(self) -> List[tuple]:
-        """the records a drop-mode decoder (TFR_F_DROP_MALFORMED) cut out of this batch, in record order (tfr_batch_dropped):
+        """the records a drop-mode decoder (TFR_F_DROP_MALFORMED) cut out of this batch, or a PERMISSIVE one delivered as
+        corrupt rows, in record order (tfr_batch_dropped):
         [(frame index in the block, byte offset in the submitted buffer, TFR_E_* code, schema field or -1)]"""
         n = C.c_int64()
         _check(lib().tfr_batch_dropped(self.h, C.byref(n), None, None, None, None, 0))
@@ -326,11 +328,17 @@ class Batch:
 
 
 class Decoder:
-    def __init__(self, schema: StructType, record_type: int = 0, device: int = 0, flags: int = A.TFR_F_DEFAULT):
+    def __init__(self, schema: StructType, record_type: int = 0, device: int = 0, flags: int = A.TFR_F_DEFAULT,
+                 corrupt_field: Optional[int] = None):
+        """`corrupt_field`: with TFR_F_PERMISSIVE in `flags`, the index of the schema field that receives a failing record's
+        payload (a nullable BinaryType column; tfr_decoder_create_permissive)"""
         self.schema = Schema(schema, record_type)
         self.ncols = 1 if record_type == 2 else len(schema)
         h = C.c_void_p()
-        _check(lib().tfr_decoder_create(self.schema.h, device, flags, C.byref(h)))
+        if corrupt_field is None:
+            _check(lib().tfr_decoder_create(self.schema.h, device, flags, C.byref(h)))
+        else:
+            _check(lib().tfr_decoder_create_permissive(self.schema.h, device, flags, corrupt_field, C.byref(h)))
         self.h = h
 
     def staging(self, nbytes: int) -> np.ndarray:
@@ -350,10 +358,10 @@ class Decoder:
         return lib().tfr_decoder_num_staging_slots()
 
     def stats(self) -> dict:
-        v = (C.c_int64 * 10)()
-        _check(lib().tfr_decoder_get_stats(self.h, v, 10))
+        v = (C.c_int64 * 11)()
+        _check(lib().tfr_decoder_get_stats(self.h, v, 11))
         names = ["batches", "speculative_submits", "speculative_redone", "count_mode_batches", "general_path_batches", "shapes_learned", "transcode_reruns",
-                 "rows_async", "rows_async_rebuilt", "records_dropped"]
+                 "rows_async", "rows_async_rebuilt", "records_dropped", "records_corrupt"]
         return {k: v[i] for i, k in enumerate(names)}
 
     def stream(self) -> int:

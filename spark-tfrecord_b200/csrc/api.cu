@@ -24,6 +24,7 @@
 #include "frame.cuh"
 #include "host_util.h"
 #include "infer.cuh"
+#include "permissive.cuh"
 #include "rows.cuh"
 #include "scan.cuh"
 #include "tile.cuh"
@@ -257,6 +258,18 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
   *out = s.release();
   return TFR_OK;
 }
+// the key hash table without field `skip`: no feature of the record maps to that field any more, so every kernel writes it as
+// an absent field (a PERMISSIVE decoder's corrupt-record column)
+static void schema_rehash(tfr_schema& s, int32_t skip) {
+  std::fill(s.ht.begin(), s.ht.end(), -1);
+  const size_t mask = s.ht.size() - 1;
+  for (int32_t i = 0; i < (int32_t)s.fields.size(); ++i) {
+    if (i == skip) continue;
+    size_t slot = s.fields[i].hash & mask;
+    while (s.ht[slot] >= 0) slot = (slot + 1) & mask;
+    s.ht[slot] = i;
+  }
+}
 extern "C" void tfr_schema_destroy(tfr_schema* s) { delete s; }
 extern "C" int32_t tfr_schema_num_fields(const tfr_schema* s) { return s ? (int32_t)s->fields.size() : 0; }
 
@@ -268,7 +281,8 @@ struct DevSchemaBuf {
   DevSchema view{};
   const int32_t* d_var_field() const { return (const int32_t*)var_field.p; }
   const uint8_t* d_tile_consts() const { return (const uint8_t*)tile_consts.p; }
-  int32_t upload(const tfr_schema& s, cudaStream_t st) {
+  // `unkeyed`: a field no feature maps to (schema_rehash), which gets no entry template either
+  int32_t upload(const tfr_schema& s, cudaStream_t st, int32_t unkeyed = -1) {
     size_t nf = s.fields.size();
     CUDA_TRY(fields.alloc(std::max<size_t>(1, nf) * sizeof(DevField)));
     CUDA_TRY(names.alloc(std::max<size_t>(1, s.names.size())));
@@ -287,7 +301,7 @@ struct DevSchemaBuf {
         const DevField& fd = s.fields[f];
         t.kind = (uint32_t)fd.kind;
         const uint32_t klen = fd.name_len, total = klen + 8;
-        if (fd.kind == K_NONE || klen >= 0x80 || total > TILE_TPL_WORDS * 4) continue;      // no template: generic parse
+        if (fd.kind == K_NONE || klen >= 0x80 || total > TILE_TPL_WORDS * 4 || (int32_t)f == unkeyed) continue;      // no template: generic parse
         uint8_t bytes[TILE_TPL_WORDS * 4] = {0}, mask[TILE_TPL_WORDS * 4] = {0};
         auto put = [&](uint32_t i, uint8_t b, bool fixed) { bytes[i] = b; mask[i] = fixed ? 0xFF : 0x00; };
         put(0, 0x0A, true); put(1, 0, false); put(2, 0x0A, true); put(3, (uint8_t)klen, true);

@@ -28,8 +28,8 @@ from typing import Dict, Iterator, List, Optional, Sequence
 import numpy as np
 
 from . import _cabi, _native
-from ._cabi import TFR_F_DEFAULT, TFR_F_DROP_MALFORMED, TFR_E_BATCH_TOO_LARGE as A_TFR_E_BATCH_TOO_LARGE, columns_from_rows
-from .sqltypes import RECORD_TYPES, StructType, byte_array_schema
+from ._cabi import TFR_F_DEFAULT, TFR_F_DROP_MALFORMED, TFR_F_PERMISSIVE, TFR_E_BATCH_TOO_LARGE as A_TFR_E_BATCH_TOO_LARGE, columns_from_rows
+from .sqltypes import RECORD_TYPES, BinaryType, StructType, byte_array_schema
 
 M = "src/main/scala/com/linkedin/spark/datasources/tfrecord/"
 _LOG = logging.getLogger(__name__)
@@ -42,10 +42,17 @@ def _record_type(options: Optional[Dict[str, str]]) -> int:
     return RECORD_TYPES[rt]
 
 
-def _decoder_flags(options: Optional[Dict[str, str]]) -> int:
+def _corrupt_column_name(options: Optional[Dict[str, str]]) -> str:
+    """the option columnNameOfCorruptRecord, named and defaulted as Spark's JSON and CSV sources have it"""
+    return (options or {}).get("columnNameOfCorruptRecord", "_corrupt_record")
+
+
+def _decoder_flags(options: Optional[Dict[str, str]], dataSchema: Optional[StructType] = None) -> int:
     """the `mode` option, case-insensitive as Spark's ParseMode reads it -> decoder flags.  FAILFAST (the default, the
     reference's behaviour): the first failing record ends the file.  DROPMALFORMED: failing records are dropped and the
-    rest is read (framing errors still end the file).  PERMISSIVE needs a corrupt-record column, which this source has not."""
+    rest is read (framing errors still end the file).  PERMISSIVE: a failing record is read as a row of nulls; it needs a
+    corrupt-record column in `dataSchema` (a field named by columnNameOfCorruptRecord, nullable BinaryType), which
+    receives the record's payload, and Example or SequenceExample records."""
     mode = (options or {}).get("mode", "FAILFAST")
     m = mode.upper() if isinstance(mode, str) else mode
     if m == "FAILFAST":
@@ -53,9 +60,30 @@ def _decoder_flags(options: Optional[Dict[str, str]]) -> int:
     if m == "DROPMALFORMED":
         return TFR_F_DEFAULT | TFR_F_DROP_MALFORMED
     if m == "PERMISSIVE":
-        raise _native.IllegalArgumentException(-1, "mode PERMISSIVE is not supported: the tfrecord source has no corrupt-record "
-                                                   "column; use FAILFAST or DROPMALFORMED")
-    raise _native.IllegalArgumentException(-1, f"mode {mode}: the tfrecord source supports FAILFAST and DROPMALFORMED")
+        name = _corrupt_column_name(options)
+        field = next((f for f in dataSchema or () if f.name == name), None)
+        if field is None:
+            raise _native.IllegalArgumentException(-1, f"mode PERMISSIVE needs a corrupt-record column: the data schema has no field "
+                                                       f"'{name}' (option columnNameOfCorruptRecord); use FAILFAST or DROPMALFORMED")
+        if field.dataType != BinaryType() or not field.nullable:
+            raise _native.IllegalArgumentException(-1, f"The field for corrupt records must be binary type and nullable: '{name}' "
+                                                       f"is {field.dataType!r}{'' if field.nullable else ' NOT NULL'}")
+        if _record_type(options) == RECORD_TYPES["ByteArray"]:
+            raise _native.IllegalArgumentException(-1, "mode PERMISSIVE: ByteArray records have no corrupt-record column; "
+                                                       "use FAILFAST or DROPMALFORMED")
+        return TFR_F_DEFAULT | TFR_F_PERMISSIVE
+    raise _native.IllegalArgumentException(-1, f"mode {mode}: the tfrecord source supports FAILFAST and DROPMALFORMED, and "
+                                               f"PERMISSIVE with a corrupt-record column")
+
+
+def _read_mode(options: Optional[Dict[str, str]], dataSchema: StructType, requiredSchema: StructType):
+    """-> (decoder flags, index of the corrupt-record column in `requiredSchema` or None).  PERMISSIVE with that column
+    pruned by a projection still reads failing records, as rows of nulls (Spark's JSON source does the same)."""
+    flags = _decoder_flags(options, dataSchema)
+    if not flags & TFR_F_PERMISSIVE:
+        return flags, None
+    name = _corrupt_column_name(options)
+    return flags, next((i for i, f in enumerate(requiredSchema) if f.name == name), None)
 
 
 # ---- stream compression (SURVEY 8f.3): host-side, around the same GPU kernels -------------------------------------------
@@ -273,17 +301,19 @@ class TFRecordFileReader:
 
     @staticmethod
     def readFile(conf, options: Dict[str, str], file: PartitionedFile, schema: StructType, device: int = 0,
-                 block_bytes: Optional[int] = None) -> Iterator[tuple]:
+                 block_bytes: Optional[int] = None, dataSchema: Optional[StructType] = None) -> Iterator[tuple]:
         """Stages the file in blocks into the decoder's pinned staging slots and decodes each block on the GPU
         (tfr_decode_submit); where a block ends -- the carry into the next one -- is known as soon as its frame index has
         run (tfr_batch_consumed), so block k+1 is read and submitted while block k decodes and block k-1's rows are
         handed out.  Rows before a bad record are yielded, then the exception the reference would throw is raised.
         With options["mode"] = "DROPMALFORMED" a failing record is skipped instead (a framing error still raises), and
-        the dropped records of each block are logged once, with the file offset of the first."""
+        the dropped records of each block are logged once, with the file offset of the first.  With "PERMISSIVE" it is a
+        row of nulls, its payload in the corrupt-record column when `schema` holds it, and logged the same way.
+        `dataSchema` (default: `schema`) is the file's schema, which PERMISSIVE needs the corrupt-record column in."""
         rt = _record_type(options)
-        flags = _decoder_flags(options)
+        flags, corrupt = _read_mode(options, schema if dataSchema is None else dataSchema, schema)
         block = block_bytes or TFRecordFileReader.BLOCK_BYTES
-        dec = _native.Decoder(schema, rt, device, flags)
+        dec = _native.Decoder(schema, rt, device, flags, corrupt_field=corrupt)
 
         def gen():
             todo = []
@@ -313,12 +343,13 @@ class TFRecordFileReader:
                         try:
                             for row in _rows_of(batch):
                                 yield row
-                            if flags & TFR_F_DROP_MALFORMED:
+                            if flags & (TFR_F_DROP_MALFORMED | TFR_F_PERMISSIVE):
                                 dropped = batch.dropped()
                                 if dropped:
-                                    _LOG.warning("%s: dropped %d malformed record(s) of the block at offset %d; the first at "
-                                                 "file offset %d (%s)", file.toPath(), len(dropped), block_pos,
-                                                 block_pos + dropped[0][1], _cabi.STATUS_NAMES.get(dropped[0][2], dropped[0][2]))
+                                    _LOG.warning("%s: %s %d malformed record(s) of the block at offset %d; the first at "
+                                                 "file offset %d (%s)", file.toPath(),
+                                                 "read as corrupt rows" if flags & TFR_F_PERMISSIVE else "dropped", len(dropped),
+                                                 block_pos, block_pos + dropped[0][1], _cabi.STATUS_NAMES.get(dropped[0][2], dropped[0][2]))
                             batch.raise_if_error()
                         finally:
                             batch.release()
@@ -438,10 +469,10 @@ class DefaultSource:
         return codes_to_struct(allreduce_schema(local, dist, f"cuda:{device}" if dist is not None and dist.is_initialized() and dist.get_backend() == "nccl" else None))
 
     def buildReader(self, dataSchema: StructType, requiredSchema: StructType, options: Dict[str, str], device: int = 0):
-        """-> PartitionedFile => Iterator[row] (filters are accepted and ignored, :123).  options["mode"]: FAILFAST (default)
-        or DROPMALFORMED, checked here, before any file is read."""
-        _decoder_flags(options)
-        return lambda file: TFRecordFileReader.readFile(None, options, file, requiredSchema, device)
+        """-> PartitionedFile => Iterator[row] (filters are accepted and ignored, :123).  options["mode"]: FAILFAST (default),
+        DROPMALFORMED, or PERMISSIVE when `dataSchema` holds the corrupt-record column, checked here, before any file is read."""
+        _read_mode(options, dataSchema, requiredSchema)
+        return lambda file: TFRecordFileReader.readFile(None, options, file, requiredSchema, device, dataSchema=dataSchema)
 
     def prepareWrite(self, options: Dict[str, str], dataSchema: StructType):
         codec = _codec_name((options or {}).get("codec", ""))             # :94-102: the option turns output compression on

@@ -7,6 +7,7 @@
 //     static native long schemaCreate(String[] names, int[] elemTypes, int[] depths, boolean[] nullable, int recordType);
 //     static native void schemaDestroy(long schema);
 //     static native long decoderCreate(long schema, int device, int flags);
+//     static native long decoderCreatePermissive(long schema, int device, int flags, int corruptField);   // mode=PERMISSIVE; -1: no corrupt column
 //     static native void decoderDestroy(long decoder);    // TaskCompletionListener + the iterator's idempotent close (M/TFRecordFileReader.scala:36-40,52-57)
 //     static native java.nio.ByteBuffer decoderStaging(long decoder, int slot, long minBytes);   // direct, pinned; slots 0..stagingSlots()-1
 //     static native int stagingSlots();
@@ -16,7 +17,7 @@
 //     static native long[] batchStatus(long batch);      // {nRows, nRecords, consumed, errorCode, errorRow, errorField}; waits for a submitted batch
 //     static native java.nio.ByteBuffer[] batchColumnHost(long batch, int column, long[] meta);  // validity, offsets*, values
 //     static native void batchExportArrowDevice(long batch, int column, long arrowDeviceArrayAddr, long arrowSchemaAddr);  // ColumnarBatch on the GPU (spark-rapids)
-//     static native long[] batchDropped(long batch, int maxEntries);   // {nDropped, (record, offset, code, field)*}: DROPMALFORMED
+//     static native long[] batchDropped(long batch, int maxEntries);   // {nDropped, (record, offset, code, field)*}: DROPMALFORMED, PERMISSIVE
 //     static native void batchThrowIfError(long batch);   // the exception the reference would throw for the first failing record
 //     static native void batchRelease(long batch);
 //     static native java.nio.ByteBuffer[] batchRows(long batch);   // {rows, int64 row offsets}: pinned UnsafeRows, valid until batchRelease
@@ -85,6 +86,15 @@ extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_
 extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_decoderCreate(JNIEnv* env, jclass, jlong schema, jint device, jint flags) {
   tfr_decoder* d = nullptr;
   int32_t rc = tfr_decoder_create((const tfr_schema*)schema, device, (uint32_t)flags, &d);
+  if (rc) { throw_for(env, rc, -1); return 0; }
+  return (jlong)d;
+}
+// mode=PERMISSIVE (flags hold TFR_F_PERMISSIVE): corruptField is the corrupt-record column's index in the required schema,
+// -1 when a projection pruned it (failing records are then rows of nulls only)
+extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_decoderCreatePermissive(JNIEnv* env, jclass, jlong schema, jint device,
+                                                                                                           jint flags, jint corruptField) {
+  tfr_decoder* d = nullptr;
+  int32_t rc = tfr_decoder_create_permissive((const tfr_schema*)schema, device, (uint32_t)flags, corruptField, &d);
   if (rc) { throw_for(env, rc, -1); return 0; }
   return (jlong)d;
 }
