@@ -478,13 +478,38 @@ enum { TFR_INF_NULL = 0, TFR_INF_LONG = 1, TFR_INF_FLOAT = 2, TFR_INF_STRING = 3
        TFR_INF_ARR2_LONG = 7, TFR_INF_ARR2_FLOAT = 8, TFR_INF_ARR2_STRING = 9,
        TFR_INF_ARR2_NULL = 10 /* ArrayType(ArrayType(null)): a FeatureList whose steps are all empty (:102-107) */ };
 typedef struct tfr_infer tfr_infer;
+/* FAILFAST, the reference's inference: the first failing record fails the update call.  Same as
+ * tfr_infer_create_mode(record_type, device, 0, NULL, 0, out).                                            */
 int32_t tfr_infer_create(int32_t record_type, int32_t device, tfr_infer** out);
+/* Inference in one of the decoder's parse modes.  flags: 0 or TFR_F_VERIFY_CRC (FAILFAST; inference always verifies
+ * the data CRC), TFR_F_DROP_MALFORMED or TFR_F_PERMISSIVE (either with TFR_F_VERIFY_CRC).  In the two tolerant modes a
+ * record error -- TFR_E_CRC_DATA, TFR_E_MALFORMED_PROTO, TFR_E_KIND_MISMATCH (kind not set), TFR_E_EMPTY_SCALAR (a
+ * FeatureList without steps), judged as FAILFAST judges them -- skips the record, which contributes nothing: none of its
+ * names, no code, no ArrayType(ArrayType(null)) flag.  A record that does not fail contributes what it does in FAILFAST.
+ * Framing errors (TFR_E_CRC_LENGTH, TFR_E_TRUNCATED, TFR_E_RECORD_TOO_LARGE) still fail the call after the names of the
+ * records before the stop are merged.  Limits of the device tables (more than 1,024 entries in one map, more than 65,536
+ * names, a name of 16 MiB or more) still fail the call with TFR_E_BATCH_TOO_LARGE, unless the record over a limit fails
+ * its CRC or its parse: then it is skipped.  The ArrayType(ArrayType(null)) conflict of tfr_infer_result is judged over
+ * the kept records.  PERMISSIVE takes the corrupt-record column's name (corrupt_name_len bytes, 1 .. 2^24 - 1): an
+ * entry of that key, in features / context or in feature_lists, is parsed but never merged, and its value errors do not
+ * fail the record, as the decoder never looks that name up; in DROPMALFORMED it is an ordinary name.  TFR_E_INVALID_ARG,
+ * before any device work, for both mode flags, unknown flag bits, a name without TFR_F_PERMISSIVE, or PERMISSIVE without
+ * a name or with a length out of range; TFR_RT_BYTE_ARRAY is TFR_E_BAD_RECORD_TYPE as for tfr_infer_create.          */
+int32_t tfr_infer_create_mode(int32_t record_type, int32_t device, uint32_t flags,
+                              const char* corrupt_name, int32_t corrupt_name_len, tfr_infer** out);
 /* accumulate one block of framed bytes (seqOp of rdd.aggregate, :40,43).  tfr_infer_update takes a whole
  * file (a trailing partial record is TFR_E_TRUNCATED); tfr_infer_update_block streams a file of any size in
  * blocks below 2 GiB with the tfr_decode contract (is_final / *consumed).                                  */
 int32_t tfr_infer_update(tfr_infer*, const void* data, size_t nbytes, int32_t data_on_device);
 int32_t tfr_infer_update_block(tfr_infer*, const void* data, size_t nbytes, int32_t data_on_device,
                                int32_t is_final, size_t* consumed);
+/* The records the last update call skipped (tolerant modes), in the shape of tfr_batch_dropped: *n_skipped is their
+ * number and the first min(*n_skipped, cap) entries are filled in record order with the frame index within the
+ * submitted block, the frame's byte offset in the submitted buffer and the TFR_E_* code (the field is always -1, so
+ * there is no field array).  The arrays may be NULL when cap = 0.  After a call that failed with a framing error the list
+ * holds the records skipped before the stop; after any other failing call, and always in FAILFAST, it is empty.       */
+int32_t tfr_infer_skipped(tfr_infer*, int64_t* n_skipped, int64_t* record, int64_t* offset,
+                          int32_t* code, int64_t cap);
 /* number of distinct feature names seen so far, then the (name, code) pairs; names are
  * returned sorted bytewise so that ranks can merge them deterministically               */
 int32_t tfr_infer_result(tfr_infer*, int32_t* n_names);

@@ -29,7 +29,8 @@ EXPORTS = [
     "tfr_encoder_create", "tfr_encoder_destroy", "tfr_encode", "tfr_encoder_row_staging", "tfr_encode_rows", "tfr_encoder_result_host",
     "tfr_encoder_stream", "tfr_encoder_num_row_slots", "tfr_encoder_row_staging_slot", "tfr_encode_rows_submit", "tfr_encoded_wait",
     "tfr_encoded_result", "tfr_encoded_release", "tfr_encoder_get_stats",
-    "tfr_infer_create", "tfr_infer_update", "tfr_infer_update_block", "tfr_infer_result", "tfr_infer_name", "tfr_infer_destroy",
+    "tfr_infer_create", "tfr_infer_create_mode", "tfr_infer_update", "tfr_infer_update_block", "tfr_infer_skipped",
+    "tfr_infer_result", "tfr_infer_name", "tfr_infer_destroy",
 ]
 
 
@@ -146,6 +147,8 @@ def lib():
         "tfr_encoded_release": (None, [vp]),
         "tfr_encoder_get_stats": (i32, [vp, P(i64), i32]),
         "tfr_infer_create": (i32, [i32, i32, P(vp)]),
+        "tfr_infer_create_mode": (i32, [i32, i32, u32, C.c_char_p, i32, P(vp)]),
+        "tfr_infer_skipped": (i32, [vp, P(i64), P(i64), P(i64), P(i32), i64]),
         "tfr_infer_update": (i32, [vp, vp, sz, i32]),
         "tfr_infer_result": (i32, [vp, P(i32)]),
         "tfr_infer_name": (i32, [vp, i32, P(C.c_char_p), P(i32), P(i32)]),
@@ -578,11 +581,15 @@ class Encoded:
 
 class Infer:
     """Schema inference accumulator (tfr_infer_*): update() is the seqOp over one block of framed bytes, result()
-    the merged name -> lattice code map (TFR_INF_*)."""
+    the merged name -> lattice code map (TFR_INF_*).  `flags` picks the parse mode (0: FAILFAST; TFR_F_DROP_MALFORMED or
+    TFR_F_PERMISSIVE skip failing records, see skipped()); PERMISSIVE takes the corrupt-record column's name, which
+    inference ignores in every record (tfr_infer_create_mode)."""
 
-    def __init__(self, record_type: int = 0, device: int = 0):
+    def __init__(self, record_type: int = 0, device: int = 0, flags: int = 0, corrupt_name=None):
         h = C.c_void_p()
-        _check(lib().tfr_infer_create(record_type, device, C.byref(h)))
+        self.h = None
+        name = corrupt_name.encode() if isinstance(corrupt_name, str) else corrupt_name
+        _check(lib().tfr_infer_create_mode(record_type, device, flags, name, len(name) if name is not None else 0, C.byref(h)))
         self.h = h
 
     def update(self, data):
@@ -597,6 +604,18 @@ class Infer:
         used = C.c_size_t()
         _check(lib().tfr_infer_update_block(self.h, ptr, n, on_dev, 1 if is_final else 0, C.byref(used)))
         return used.value
+
+    def skipped(self) -> List[tuple]:
+        """the records the last update call skipped, in record order (tfr_infer_skipped), shaped like Batch.dropped():
+        [(frame index in the block, byte offset in the submitted buffer, TFR_E_* code, -1)]"""
+        n = C.c_int64()
+        _check(lib().tfr_infer_skipped(self.h, C.byref(n), None, None, None, 0))
+        k = n.value
+        if k == 0:
+            return []
+        rec, off, code = (C.c_int64 * k)(), (C.c_int64 * k)(), (C.c_int32 * k)()
+        _check(lib().tfr_infer_skipped(self.h, C.byref(n), rec, off, code, k))
+        return [(rec[i], off[i], code[i], -1) for i in range(k)]
 
     def result(self) -> dict:
         n = C.c_int32()

@@ -12,6 +12,11 @@
 // A record's verdict is the reference's: a CRC or parse failure anywhere in the record (parseFrom throws before
 // inference sees a value), else the first value error of the surviving entries in map order (the position of a key's
 // first occurrence), context before feature_lists.
+// infer_kernel<false> is FAILFAST: a failing record fails the call, so each map's clean survivors are merged as soon as the
+// map is de-duplicated.  infer_kernel<true> serves DROPMALFORMED and PERMISSIVE, which skip a failing record: the merge is
+// record-atomic -- every map of the record stays in shared memory (a SequenceExample has a second window per warp for its
+// feature_lists) until the verdict is known, and only a clean record's survivors reach the table.  In PERMISSIVE an entry
+// named like the corrupt-record column (A.corrupt) is parsed but neither merged nor a value error.
 #pragma once
 #include "common.cuh"
 #include "decode.cuh"
@@ -25,10 +30,12 @@ struct InferSlot {
 };
 #define INFER_TABLE_SLOTS 65536u
 #define INFER_MAX_ENT 1024     // entries of one map buffered per record for last-wins de-duplication; more raise INF_OVF_ENTRIES
+static_assert(INFER_MAX_ENT <= 32 * 32, "infer_kernel<true> keeps one bit per entry of a lane in a 32-bit mask");
 #define INFER_CLAIMED (~0ull)  // a slot whose name is being written: its hash is published after the name
 enum { INF_OVF_TABLE = 1u, INF_OVF_ENTRIES = 2u, INF_OVF_KEY = 4u };   // limits hit: reported as an explicit error, never as a silently wrong schema
-// per-entry record in shared memory: ecode = lattice code (bits 0-3) | value error (bits 4-7, INF_ERR_*) | key length << 8
-enum { INF_ERR_KIND = 1u, INF_ERR_EMPTY = 2u };
+// per-entry record in shared memory: ecode = lattice code (bits 0-3) | value error (bits 4-7, INF_ERR_*) | key length << 8.
+// infer_kernel<true> only: INF_ERR_IGNORED marks an entry of the corrupt-record column's name.
+enum { INF_ERR_KIND = 1u, INF_ERR_EMPTY = 2u, INF_ERR_IGNORED = 4u };
 
 struct InferArgs {
   const uint8_t* data;
@@ -40,9 +47,13 @@ struct InferArgs {
   InferSlot* table;
   uint32_t* first_err;       // [0] min failing record index, [1] INF_OVF_* flags, [4] min record index over a per-record limit
   uint32_t* status;          // [n]
+  // PERMISSIVE (infer_kernel<true>): the corrupt-record column's name, its hash64; corrupt_len = 0 otherwise
+  const uint8_t* corrupt;
+  unsigned long long corrupt_hash;
+  uint32_t corrupt_len;
 };
 
-__device__ __forceinline__ unsigned long long hash64(const uint8_t* p, uint32_t n) {
+__host__ __device__ __forceinline__ unsigned long long hash64(const uint8_t* p, uint32_t n) {
   unsigned long long h = 1469598103934665603ull;
   for (uint32_t i = 0; i < n; ++i) h = (h ^ p[i]) * 1099511628211ull;
   return (h == 0ull || h == INFER_CLAIMED) ? 1ull : h;          // 0 and INFER_CLAIMED mark slots
@@ -93,6 +104,7 @@ __device__ __forceinline__ void infer_merge(InferSlot* table, const uint8_t* dat
 
 // one map (Features or FeatureLists) of one record: entries -> (hash, code | value error, key) in shared memory.  Returns
 // false when the map does not parse; `over` is set when the map passes a per-record limit (entries, key length).
+template <bool TOL>
 __device__ __forceinline__ bool infer_map(const InferArgs& A, Cur body, bool is_flist, unsigned long long* eh, uint32_t* ecode, uint32_t* ekey,
                                           uint32_t& nent, bool& over) {
   const uint32_t lane = threadIdx.x & 31;
@@ -145,6 +157,9 @@ __device__ __forceinline__ bool infer_map(const InferArgs& A, Cur body, bool is_
         else if (step_unset) verr = INF_ERR_KIND;
         else if (fl_code == 0) code = 10;                                               // ArrayType(ArrayType(null))
         else code = 7 + (fl_code - 1) % 3;                                              // T or [T] -> [[T]]
+        if constexpr (TOL) {
+          if (klen == A.corrupt_len && h == A.corrupt_hash && bytes_equal(key, A.corrupt, klen)) { code = 0; verr = INF_ERR_IGNORED; }
+        }
       }
     }
     if (__any_sync(FULLMASK, !ok)) return false;
@@ -181,12 +196,18 @@ __device__ __forceinline__ bool same_key(const uint8_t* data, const unsigned lon
   return eh[i] == eh[j] && (ecode[i] >> 8) == (ecode[j] >> 8) && bytes_equal(data + ekey[i], data + ekey[j], ecode[i] >> 8);
 }
 
+// shared memory of one launch: the CRC tables, then per warp one window of INFER_MAX_ENT entries per map kept at once
+__host__ __device__ constexpr uint32_t infer_windows(bool tol, uint32_t record_type) { return tol && record_type == TFR_RT_SEQUENCE_EXAMPLE ? 2u : 1u; }
+#define INFER_WINDOW_BYTES (INFER_MAX_ENT * 16)
+
+template <bool TOL>
 __global__ void __launch_bounds__(128) infer_kernel(InferArgs A) {
   extern __shared__ uint32_t smem[];
   uint32_t* stab = smem;
   crc_stage_tables(stab, A.tabs);
   const uint32_t warps = blockDim.x >> 5, wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint8_t* wbase = reinterpret_cast<uint8_t*>(smem + CRC_SMEM_WORDS) + (size_t)wid * INFER_MAX_ENT * 16;
+  const uint32_t nwin = infer_windows(TOL, A.record_type);
+  uint8_t* wbase = reinterpret_cast<uint8_t*>(smem + CRC_SMEM_WORDS) + (size_t)wid * nwin * INFER_WINDOW_BYTES;
   unsigned long long* eh = reinterpret_cast<unsigned long long*>(wbase);
   uint32_t* ecode = reinterpret_cast<uint32_t*>(wbase + INFER_MAX_ENT * 8);
   uint32_t* ekey = reinterpret_cast<uint32_t*>(wbase + INFER_MAX_ENT * 12);
@@ -199,9 +220,16 @@ __global__ void __launch_bounds__(128) infer_kernel(InferArgs A) {
     if (A.verify && crc_mask(crc_warp(stab, payload, len)) != load_u32_unaligned(payload + len)) err = TFR_E_CRC_DATA;
     bool ok = true, over = false;
     uint32_t verr = 0;         // the record's first value error (INF_ERR_*): context's before feature_lists'
+    // infer_kernel<true>: per map, bit k set when entry lane + 32 k is a clean survivor (registers, not shared memory)
+    uint32_t keep0 = 0u, keep1 = 0u;
     // pass 0: features/context (field 1), pass 1: feature_lists (field 2).  Both are parsed before a value error counts.
     for (int pass = 0; pass < 2 && ok && !err; ++pass) {
       if (pass == 1 && A.record_type != TFR_RT_SEQUENCE_EXAMPLE) break;
+      if constexpr (TOL) {       // each map in its own window: nothing is merged before the record's verdict
+        eh = reinterpret_cast<unsigned long long*>(wbase + pass * INFER_WINDOW_BYTES);
+        ecode = reinterpret_cast<uint32_t*>(wbase + pass * INFER_WINDOW_BYTES + INFER_MAX_ENT * 8);
+        ekey = reinterpret_cast<uint32_t*>(wbase + pass * INFER_WINDOW_BYTES + INFER_MAX_ENT * 12);
+      }
       uint32_t nent = 0;
       Cur top{payload, payload + len};
       for (;;) {
@@ -211,7 +239,7 @@ __global__ void __launch_bounds__(128) infer_kernel(InferArgs A) {
         if (tag == 0x0A || (tag == 0x12 && A.record_type == TFR_RT_SEQUENCE_EXAMPLE)) {
           uint32_t l;
           if (!rd_len(top, l)) { ok = false; break; }
-          if ((tag == 0x0A) == (pass == 0) && !infer_map(A, Cur{top.p, top.p + l}, pass == 1, eh, ecode, ekey, nent, over)) { ok = false; break; }
+          if ((tag == 0x0A) == (pass == 0) && !infer_map<TOL>(A, Cur{top.p, top.p + l}, pass == 1, eh, ecode, ekey, nent, over)) { ok = false; break; }
           top.p += l;
         } else if (!skip_field(top, tag)) { ok = false; break; }
       }
@@ -221,6 +249,9 @@ __global__ void __launch_bounds__(128) infer_kernel(InferArgs A) {
       // of the key's first occurrence, which orders the value errors
       uint32_t first_err = 0xffffffffu;     // (first-occurrence position << 8) | INF_ERR_*
       for (uint32_t i = lane; i < nent; i += 32) {
+        if constexpr (TOL) {
+          if ((ecode[i] >> 4) & INF_ERR_IGNORED) continue;      // (so is every entry of its key)
+        }
         bool last = true;
         for (uint32_t j = i + 1; j < nent; ++j) if (same_key(A.data, eh, ecode, ekey, i, j)) { last = false; break; }
         if (!last) continue;
@@ -229,6 +260,8 @@ __global__ void __launch_bounds__(128) infer_kernel(InferArgs A) {
           uint32_t pos = i;
           for (uint32_t j = 0; j < i; ++j) if (same_key(A.data, eh, ecode, ekey, i, j)) { pos = j; break; }
           first_err = min(first_err, (pos << 8) | e);
+        } else if constexpr (TOL) {
+          (pass ? keep1 : keep0) |= 1u << (i >> 5);              // merged below if the record is kept
         } else {
           infer_merge(A.table, A.data, eh[i], ekey[i], ecode[i] >> 8, (int)(ecode[i] & 0xf), &A.first_err[1]);
         }
@@ -238,12 +271,27 @@ __global__ void __launch_bounds__(128) infer_kernel(InferArgs A) {
       __syncwarp();
     }
     over = __any_sync(FULLMASK, over);
-    // a record that fails spoils the whole call, so what it merged into the table before failing is never read
+    // FAILFAST: a record that fails spoils the whole call, so what it merged into the table before failing is never read
     uint32_t st = 0;
     if (err) st = make_status(err, -1);
     else if (!ok) st = make_status(TFR_E_MALFORMED_PROTO, -1);
     else if (over) { if (lane == 0) atomicMin(&A.first_err[4], row); }   // its entries past the window decide: unknown here
     else if (verr) st = make_status(verr == INF_ERR_KIND ? TFR_E_KIND_MISMATCH : TFR_E_EMPTY_SCALAR, -1);
+    if constexpr (TOL) {
+      if (!st && !over) {        // the record is kept: its clean survivors, context then feature_lists
+        for (uint32_t w = 0; w < nwin; ++w) {
+          const uint8_t* wb = wbase + w * INFER_WINDOW_BYTES;
+          const unsigned long long* wh = reinterpret_cast<const unsigned long long*>(wb);
+          const uint32_t* wc = reinterpret_cast<const uint32_t*>(wb + INFER_MAX_ENT * 8);
+          const uint32_t* wk = reinterpret_cast<const uint32_t*>(wb + INFER_MAX_ENT * 12);
+          for (uint32_t m = w ? keep1 : keep0; m; m &= m - 1) {
+            const uint32_t i = lane + 32u * (uint32_t)__ffs(m) - 32u;
+            infer_merge(A.table, A.data, wh[i], wk[i], wc[i] >> 8, (int)(wc[i] & 0xf), &A.first_err[1]);
+          }
+        }
+      }
+      __syncwarp();              // the windows are rewritten by the warp's next record
+    }
     if (lane == 0) { A.status[row] = st; if (st) atomicMin(&A.first_err[0], row); }
   }
 }

@@ -29,7 +29,7 @@ import numpy as np
 
 from . import _cabi, _native
 from ._cabi import TFR_F_DEFAULT, TFR_F_DROP_MALFORMED, TFR_F_PERMISSIVE, TFR_E_BATCH_TOO_LARGE as A_TFR_E_BATCH_TOO_LARGE, columns_from_rows
-from .sqltypes import RECORD_TYPES, BinaryType, StructType, byte_array_schema
+from .sqltypes import RECORD_TYPES, BinaryType, StructField, StructType, byte_array_schema
 
 M = "src/main/scala/com/linkedin/spark/datasources/tfrecord/"
 _LOG = logging.getLogger(__name__)
@@ -47,14 +47,23 @@ def _corrupt_column_name(options: Optional[Dict[str, str]]) -> str:
     return (options or {}).get("columnNameOfCorruptRecord", "_corrupt_record")
 
 
-def _decoder_flags(options: Optional[Dict[str, str]], dataSchema: Optional[StructType] = None) -> int:
-    """the `mode` option, case-insensitive as Spark's ParseMode reads it -> decoder flags.  FAILFAST (the default, the
-    reference's behaviour): the first failing record ends the file.  DROPMALFORMED: failing records are dropped and the
-    rest is read (framing errors still end the file).  PERMISSIVE: a failing record is read as a row of nulls; it needs a
-    corrupt-record column in `dataSchema` (a field named by columnNameOfCorruptRecord, nullable BinaryType), which
-    receives the record's payload, and Example or SequenceExample records."""
+def _parse_mode(options: Optional[Dict[str, str]]) -> str:
+    """the `mode` option, case-insensitive as Spark's ParseMode reads it -> FAILFAST, DROPMALFORMED or PERMISSIVE"""
     mode = (options or {}).get("mode", "FAILFAST")
     m = mode.upper() if isinstance(mode, str) else mode
+    if m in ("FAILFAST", "DROPMALFORMED", "PERMISSIVE"):
+        return m
+    raise _native.IllegalArgumentException(-1, f"mode {mode}: the tfrecord source supports FAILFAST and DROPMALFORMED, and "
+                                               f"PERMISSIVE with a corrupt-record column")
+
+
+def _decoder_flags(options: Optional[Dict[str, str]], dataSchema: Optional[StructType] = None) -> int:
+    """the `mode` option -> decoder flags.  FAILFAST (the default, the reference's behaviour): the first failing record
+    ends the file.  DROPMALFORMED: failing records are dropped and the rest is read (framing errors still end the file).
+    PERMISSIVE: a failing record is read as a row of nulls; it needs a corrupt-record column in `dataSchema` (a field
+    named by columnNameOfCorruptRecord, nullable BinaryType), which receives the record's payload, and Example or
+    SequenceExample records."""
+    m = _parse_mode(options)
     if m == "FAILFAST":
         return TFR_F_DEFAULT
     if m == "DROPMALFORMED":
@@ -72,8 +81,6 @@ def _decoder_flags(options: Optional[Dict[str, str]], dataSchema: Optional[Struc
             raise _native.IllegalArgumentException(-1, "mode PERMISSIVE: ByteArray records have no corrupt-record column; "
                                                        "use FAILFAST or DROPMALFORMED")
         return TFR_F_DEFAULT | TFR_F_PERMISSIVE
-    raise _native.IllegalArgumentException(-1, f"mode {mode}: the tfrecord source supports FAILFAST and DROPMALFORMED, and "
-                                               f"PERMISSIVE with a corrupt-record column")
 
 
 def _read_mode(options: Optional[Dict[str, str]], dataSchema: StructType, requiredSchema: StructType):
@@ -437,18 +444,28 @@ class DefaultSource:
     def inferSchema(self, options: Dict[str, str], files: Sequence[str], device: int = 0, dist=None):
         """M/DefaultSource.scala:31-39,48-70: the first non-empty file is scanned (the reference scans it twice);
         ByteArray has the fixed one-column schema.  With `dist`, every rank scans its shard of the files and the maps
-        are merged with one all-reduce (sharding.allreduce_schema)."""
+        are merged with one all-reduce (sharding.allreduce_schema).
+        options["mode"] as the reader takes it: FAILFAST (default) fails on the first failing record.  DROPMALFORMED and
+        PERMISSIVE skip failing records (framing errors still fail), logging them once per file, and without `dist` take
+        the first file whose records give any name (the reference's collectFirst(hasSchema), M/DefaultSource.scala:36-38),
+        since a file of skipped records only would give an empty schema.  PERMISSIVE ignores features named by
+        columnNameOfCorruptRecord and always ends the schema with that column (nullable BinaryType), so that the schema
+        reads the files back under the options it was inferred with (buildReader refuses PERMISSIVE without it)."""
         from .sharding import allreduce_schema, codes_to_struct, shard_lpt
+        mode = _parse_mode(options)
         rt = _record_type(options)
         if rt == 2:
             return byte_array_schema()
+        corrupt = _corrupt_column_name(options) if mode == "PERMISSIVE" else None
+        flags = {"FAILFAST": 0, "DROPMALFORMED": TFR_F_DEFAULT | TFR_F_DROP_MALFORMED, "PERMISSIVE": TFR_F_DEFAULT | TFR_F_PERMISSIVE}[mode]
+        distributed = dist is not None and dist.is_initialized()
         todo = [f for f in files if os.path.getsize(f) > 0]
-        if dist is None or not dist.is_initialized():
-            todo = todo[:1]
-        else:
+        if distributed:
             mine = shard_lpt([os.path.getsize(f) for f in todo], dist.get_world_size())[dist.get_rank()]
             todo = [todo[i] for i in mine]
-        inf = _native.Infer(rt, device)
+        elif mode == "FAILFAST":
+            todo = todo[:1]
+        inf = _native.Infer(rt, device, flags, corrupt)
         block = TFRecordFileReader.BLOCK_BYTES
         buf = [np.empty(0, dtype=np.uint8)]
 
@@ -459,14 +476,30 @@ class DefaultSource:
 
         try:
             for f in todo:                       # streamed in blocks like readFile: files of any size, no whole-file copy
+                pos, skipped = [0], []           # where the next block starts in the (decompressed) file; (file offset, code)
+
+                def process(st, nb, final):
+                    used = inf.update_block(st, final, nb)
+                    skipped.extend((pos[0] + off, code) for _, off, code, _ in inf.skipped())
+                    pos[0] += used
+                    return used
+
                 with _open_read(f) as fh:
                     remaining = (1 << 62) if _codec_of_path(f) is not None else os.path.getsize(f)
-                    for _ in _stream_blocks(fh, remaining, block, stage, lambda st, nb, final: inf.update_block(st, final, nb)):
+                    for _ in _stream_blocks(fh, remaining, block, stage, process):
                         pass
+                if skipped:
+                    _LOG.warning("%s: schema inference skipped %d malformed record(s); the first at file offset %d (%s)", f,
+                                 len(skipped), skipped[0][0], _cabi.STATUS_NAMES.get(skipped[0][1], skipped[0][1]))
+                if mode != "FAILFAST" and not distributed and inf.result():
+                    break                        # the first file whose kept records give a name
             local = inf.result()
         finally:
             inf.close()
-        return codes_to_struct(allreduce_schema(local, dist, f"cuda:{device}" if dist is not None and dist.is_initialized() and dist.get_backend() == "nccl" else None))
+        schema = codes_to_struct(allreduce_schema(local, dist, f"cuda:{device}" if distributed and dist.get_backend() == "nccl" else None))
+        if corrupt is not None:
+            schema = StructType(list(schema.fields) + [StructField(corrupt, BinaryType(), True)])
+        return schema
 
     def buildReader(self, dataSchema: StructType, requiredSchema: StructType, options: Dict[str, str], device: int = 0):
         """-> PartitionedFile => Iterator[row] (filters are accepted and ignored, :123).  options["mode"]: FAILFAST (default),

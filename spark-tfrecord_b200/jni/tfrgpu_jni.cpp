@@ -346,6 +346,34 @@ extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_
   if (rc) { throw_for(env, rc, -1); return 0; }
   return (jlong)h;
 }
+// mode=DROPMALFORMED / PERMISSIVE (flags TFR_F_DROP_MALFORMED / TFR_F_PERMISSIVE): failing records are skipped.  corruptName:
+// PERMISSIVE's columnNameOfCorruptRecord, its UTF-8 bytes in a direct ByteBuffer of corruptNameLen bytes (standard UTF-8,
+// which GetStringUTFChars does not give for every name), ignored in every record; null and 0 in the other modes.
+extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_inferCreateMode(JNIEnv* env, jclass, jint recordType, jint device,
+                                                                                                     jint flags, jobject corruptName, jint corruptNameLen) {
+  const char* name = corruptName ? (const char*)env->GetDirectBufferAddress(corruptName) : nullptr;
+  tfr_infer* h = nullptr;
+  int32_t rc = tfr_infer_create_mode(recordType, device, (uint32_t)flags, name, (int32_t)corruptNameLen, &h);
+  if (rc) { throw_for(env, rc, -1); return 0; }
+  return (jlong)h;
+}
+// The records the last inferUpdate skipped: {nSkipped, then per skipped record up to maxEntries of them record, offset, code,
+// field (always -1)}, the shape of batchDropped.  inferSchema logs the count and the first record's file offset (block offset
+// + offset) once per file.
+extern "C" JNIEXPORT jlongArray JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_inferSkipped(JNIEnv* env, jclass, jlong infer, jint maxEntries) {
+  int64_t n = 0;
+  int32_t rc = tfr_infer_skipped((tfr_infer*)infer, &n, nullptr, nullptr, nullptr, 0);
+  if (rc) { throw_for(env, rc, -1); return nullptr; }
+  const int64_t k = maxEntries < 0 ? 0 : (n < maxEntries ? n : (int64_t)maxEntries);
+  std::vector<int64_t> rec(k), off(k);
+  std::vector<int32_t> code(k);
+  if (k) tfr_infer_skipped((tfr_infer*)infer, &n, rec.data(), off.data(), code.data(), k);
+  std::vector<jlong> v(1 + 4 * k);
+  v[0] = (jlong)n;
+  for (int64_t i = 0; i < k; ++i) { v[1 + 4 * i] = rec[i]; v[2 + 4 * i] = off[i]; v[3 + 4 * i] = code[i]; v[4 + 4 * i] = -1; }
+  jlongArray a = env->NewLongArray((jsize)v.size()); env->SetLongArrayRegion(a, 0, (jsize)v.size(), v.data());
+  return a;
+}
 extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_inferUpdate(JNIEnv* env, jclass, jlong infer, jobject block, jlong nbytes, jboolean isFinal) {
   size_t used = 0;
   int32_t rc = tfr_infer_update_block((tfr_infer*)infer, env->GetDirectBufferAddress(block), (size_t)nbytes, 0, isFinal ? 1 : 0, &used);
