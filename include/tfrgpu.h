@@ -105,8 +105,8 @@ int32_t tfr_schema_num_fields(const tfr_schema*);
  * at it).  Record errors are TFR_E_CRC_DATA, TFR_E_MALFORMED_PROTO, TFR_E_KIND_MISMATCH, TFR_E_EMPTY_SCALAR,
  * TFR_E_NULL_IN_NONNULL and TFR_E_BAD_NESTING: a dropped record's length CRC verified, so the next frame is known.  The
  * batch's rows, columns, null counts and UnsafeRows are those of the block with the dropped frames cut out.  Framing errors
- * (TFR_E_CRC_LENGTH, TFR_E_TRUNCATED, TFR_E_RECORD_TOO_LARGE) still end the block, as without the flag: the frame chain is
- * lost there.  tfr_batch_info in drop mode: n_rows = the rows delivered; n_records = the frames in the consumed bytes,
+ * (TFR_E_CRC_LENGTH, TFR_E_TRUNCATED, TFR_E_RECORD_TOO_LARGE) still end the block, as without the flag: without
+ * TFR_F_RESYNC the frame chain is lost there.  tfr_batch_info in drop mode: n_rows = the rows delivered; n_records = the frames in the consumed bytes,
  * dropped ones included; consumed_bytes = what tfr_batch_consumed returns; error_code / error_row / error_field are set
  * for a framing error only, and error_row is then the frame index at which framing stopped, which can exceed n_rows by the
  * records dropped before it.  tfr_batch_dropped lists the dropped records.  Without TFR_F_VERIFY_CRC no CRC is checked,
@@ -124,6 +124,36 @@ int32_t tfr_schema_num_fields(const tfr_schema*);
  * tfr_batch_dropped lists the records delivered as corrupt rows (the frame index is the row index).  Example and
  * SequenceExample only; with TFR_F_DROP_MALFORMED or for TFR_RT_BYTE_ARRAY the create call returns TFR_E_INVALID_ARG.  */
 #define TFR_F_PERMISSIVE   0x4u
+/* Resynchronise after a framing error (DROPMALFORMED and PERMISSIVE; without this flag the frame chain is lost at a framing
+ * error and there is no resynchronisation).  Valid only together with TFR_F_VERIFY_CRC and one of TFR_F_DROP_MALFORMED or
+ * TFR_F_PERMISSIVE; any other combination is TFR_E_INVALID_ARG, before any device work.  `end` is the size of the block and
+ * H = 2^31 - 1, the largest block a decoder takes.
+ *   1. Framing stops at offset o when the header at o fails its length CRC, or its length is above INT32_MAX, or -- on the
+ *      final block only -- the frame at o is truncated (8..11 bytes left, or the frame runs past end).  1..7 stray bytes at
+ *      EOF stay a clean end; on a non-final block a partial frame stays the ordinary carry.
+ *   2. The RESYNC POINT is the smallest p > o with p + 12 <= end, the masked CRC-32C of data[p, p+8) equal to the u32 at p+8,
+ *      L = u64 at p <= INT32_MAX, p + 16 + L <= end, the payload CRC verified, and p + 16 + L - o <= H.  Framing goes on at p
+ *      as from a record boundary.
+ *   3. The LOST REGION is [o, p); on the final block without a resync point it is [o, end) and the batch ends cleanly.
+ *   4. The result does not depend on where blocks are cut.  On a non-final block a position p > o is UNDECIDED when
+ *      p + 16 <= o + H and either p + 12 > end, or its header verifies and its frame ends past end but within H of o.  When
+ *      an undecided position comes before any resync point the region is UNRESOLVED: the batch ends at o (consumed = o, the
+ *      rows before o are delivered, nothing is reported about the region) and the caller's next block starts at o with more
+ *      bytes, as in front of a large record.  A block of H bytes from o always decides; on such a block a region without a
+ *      resync point within H (some 2 GiB of damage) stays unresolved, as a record larger than H would.
+ *   5. A batch's ENTRIES are its frames and its lost regions, in byte order.  n_records counts entries; tfr_batch_dropped
+ *      lists a region with record = its entry index, offset = o, the framing code (TFR_E_CRC_LENGTH, TFR_E_RECORD_TOO_LARGE or
+ *      TFR_E_TRUNCATED) and field = -1.  DROPMALFORMED drops a region; PERMISSIVE reads it as one corrupt row at its place
+ *      (entry index = row index), data fields null, its corrupt-record column holding data[o, p) as it is, header included.
+ *      error_code is never a framing code under the flag.
+ *   6. Record errors are unchanged: a frame whose header verifies but whose payload CRC fails is a record error and its
+ *      length is trusted.  So a record cut off by a truncation and followed by a concatenated file swallows the records of
+ *      that file that lie inside its claimed length; the rule resyncs after them.
+ * Batches without a framing error take the ordinary paths (pipelined submits stay free of host synchronisation; the chains of
+ * the frame index verify every header); a pipelined batch whose frame index stopped on a framing error is resolved through
+ * the synchronous path, by tfr_batch_consumed too, since its consumed count depends on it.  tfr_decoder_get_stats counts the
+ * lost regions ([11]) and their bytes ([12]); counters [9] and [10] count records only.                                  */
+#define TFR_F_RESYNC       0x8u
 #define TFR_F_DEFAULT      (TFR_F_VERIFY_CRC)
 
 /* Replaces TFRecordFileReader.readFile's setup (M/TFRecordFileReader.scala:16-44):
@@ -197,8 +227,9 @@ int32_t tfr_decoder_get_profile(tfr_decoder*, double* ms /* [TFR_PROFILE_STAGES]
  * UTF-8 in a string column), [7] rows passes enqueued by tfr_batch_rows_async without a host synchronisation, [8] of
  * those rebuilt through the synchronous rows path (the batch was redone, or the rows did not fit what they were
  * launched with), [9] records dropped (TFR_F_DROP_MALFORMED), [10] records delivered as corrupt rows
- * (TFR_F_PERMISSIVE).  A caller passing n = 8 gets the first eight; n <= 11 gets them all, counter [10] being
- * PERMISSIVE's, and a caller passing 10 or fewer is unaffected.                                                     */
+ * (TFR_F_PERMISSIVE), [11] lost regions and [12] the bytes in them (TFR_F_RESYNC).  A caller passing n = 8 gets the
+ * first eight.  The counters before [11] keep their meaning: n <= 11 gets them all, counter [10] being PERMISSIVE's, and a
+ * caller passing 10 or fewer is unaffected; n = 13 adds the two of TFR_F_RESYNC.                                     */
 int32_t tfr_decoder_get_stats(tfr_decoder*, int64_t* out, int32_t n /* <= 10 */);
 
 int32_t tfr_batch_wait(tfr_batch*);
@@ -228,6 +259,10 @@ int32_t tfr_batch_consumed(tfr_batch*, size_t* consumed);
  * it delivered as corrupt rows, in the same format; their frame index is also their row index.                        */
 int32_t tfr_batch_dropped(tfr_batch*, int64_t* n_dropped, int64_t* record, int64_t* offset, int32_t* code, int32_t* field,
                           int64_t cap);
+/* tfr_batch_dropped's list plus each entry's byte length in nbytes (may be NULL): 16 + L for a frame, p - o for a lost
+ * region (TFR_F_RESYNC).                                                                                                  */
+int32_t tfr_batch_dropped_spans(tfr_batch*, int64_t* n_dropped, int64_t* record, int64_t* offset, int64_t* nbytes, int32_t* code,
+                                int32_t* field, int64_t cap);
 
 /* One output column in Arrow layout.  n_levels offset arrays (int32, Arrow list/binary
  * offsets) from the outermost (one entry per row + 1) to the innermost, then the leaf
@@ -487,13 +522,14 @@ int32_t tfr_infer_create(int32_t record_type, int32_t device, tfr_infer** out);
  * FeatureList without steps), judged as FAILFAST judges them -- skips the record, which contributes nothing: none of its
  * names, no code, no ArrayType(ArrayType(null)) flag.  A record that does not fail contributes what it does in FAILFAST.
  * Framing errors (TFR_E_CRC_LENGTH, TFR_E_TRUNCATED, TFR_E_RECORD_TOO_LARGE) still fail the call after the names of the
- * records before the stop are merged.  Limits of the device tables (more than 1,024 entries in one map, more than 65,536
+ * records before the stop are merged, unless TFR_F_RESYNC is set (with the rules of the decoder's flag): a lost region is
+ * skipped, listed by tfr_infer_skipped with its entry index, offset and framing code, and *consumed follows the same rule.  Limits of the device tables (more than 1,024 entries in one map, more than 65,536
  * names, a name of 16 MiB or more) still fail the call with TFR_E_BATCH_TOO_LARGE, unless the record over a limit fails
  * its CRC or its parse: then it is skipped.  The ArrayType(ArrayType(null)) conflict of tfr_infer_result is judged over
  * the kept records.  PERMISSIVE takes the corrupt-record column's name (corrupt_name_len bytes, 1 .. 2^24 - 1): an
  * entry of that key, in features / context or in feature_lists, is parsed but never merged, and its value errors do not
  * fail the record, as the decoder never looks that name up; in DROPMALFORMED it is an ordinary name.  TFR_E_INVALID_ARG,
- * before any device work, for both mode flags, unknown flag bits, a name without TFR_F_PERMISSIVE, or PERMISSIVE without
+ * before any device work, for both mode flags, TFR_F_RESYNC without a tolerant mode or without TFR_F_VERIFY_CRC, unknown flag bits, a name without TFR_F_PERMISSIVE, or PERMISSIVE without
  * a name or with a length out of range; TFR_RT_BYTE_ARRAY is TFR_E_BAD_RECORD_TYPE as for tfr_infer_create.          */
 int32_t tfr_infer_create_mode(int32_t record_type, int32_t device, uint32_t flags,
                               const char* corrupt_name, int32_t corrupt_name_len, tfr_infer** out);

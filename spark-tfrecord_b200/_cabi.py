@@ -31,11 +31,15 @@ TFR_E_BAD_NESTING = -18
 TFR_F_VERIFY_CRC = 0x1
 TFR_F_DROP_MALFORMED = 0x2       # mode=DROPMALFORMED: failing records are dropped, framing errors still end the block
 TFR_F_PERMISSIVE = 0x4           # mode=PERMISSIVE: a failing record is a row of nulls (its payload in the corrupt-record column)
+TFR_F_RESYNC = 0x8               # with DROPMALFORMED or PERMISSIVE: a framing error is a lost region, framing goes on at the next verified frame
 TFR_F_DEFAULT = TFR_F_VERIFY_CRC
 
 # the record errors a TFR_F_DROP_MALFORMED decoder drops (the other data errors are framing errors)
 RECORD_ERRORS = (TFR_E_CRC_DATA, TFR_E_MALFORMED_PROTO, TFR_E_KIND_MISMATCH, TFR_E_EMPTY_SCALAR, TFR_E_NULL_IN_NONNULL,
                  TFR_E_BAD_NESTING)
+
+# the framing errors: under TFR_F_RESYNC each names a lost region in tfr_batch_dropped / tfr_infer_skipped
+FRAMING_ERRORS = (TFR_E_CRC_LENGTH, TFR_E_TRUNCATED, TFR_E_RECORD_TOO_LARGE)
 
 STATUS_NAMES = {v: k for k, v in list(globals().items()) if k.startswith("TFR_E_") or k == "TFR_OK"}
 

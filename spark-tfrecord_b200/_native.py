@@ -23,7 +23,7 @@ EXPORTS = [
     "tfr_abi_version", "tfr_status_string", "tfr_last_error", "tfr_schema_create", "tfr_schema_destroy",
     "tfr_schema_num_fields", "tfr_decoder_create", "tfr_decoder_create_permissive", "tfr_decoder_destroy", "tfr_decoder_staging", "tfr_decoder_staging_slot",
     "tfr_decoder_num_staging_slots", "tfr_decode", "tfr_decode_submit",
-    "tfr_decoder_stream", "tfr_decoder_set_profiling", "tfr_decoder_get_profile", "tfr_decoder_get_stats", "tfr_batch_wait", "tfr_batch_status", "tfr_batch_consumed", "tfr_batch_dropped", "tfr_batch_num_columns", "tfr_batch_columns",
+    "tfr_decoder_stream", "tfr_decoder_set_profiling", "tfr_decoder_get_profile", "tfr_decoder_get_stats", "tfr_batch_wait", "tfr_batch_status", "tfr_batch_consumed", "tfr_batch_dropped", "tfr_batch_dropped_spans", "tfr_batch_num_columns", "tfr_batch_columns",
     "tfr_batch_to_host_async", "tfr_batch_to_host", "tfr_batch_export_arrow_host", "tfr_batch_export_arrow_device", "tfr_batch_release",
     "tfr_batch_rows", "tfr_batch_rows_with_partition", "tfr_batch_rows_async",
     "tfr_encoder_create", "tfr_encoder_destroy", "tfr_encode", "tfr_encoder_row_staging", "tfr_encode_rows", "tfr_encoder_result_host",
@@ -123,6 +123,7 @@ def lib():
         "tfr_batch_status": (i32, [vp, P(tfr_batch_info)]),
         "tfr_batch_consumed": (i32, [vp, P(C.c_size_t)]),
         "tfr_batch_dropped": (i32, [vp, P(i64), P(i64), P(i64), P(i32), P(i32), i64]),
+        "tfr_batch_dropped_spans": (i32, [vp, P(i64), P(i64), P(i64), P(i64), P(i32), P(i32), i64]),
         "tfr_batch_num_columns": (i32, [vp]),
         "tfr_batch_columns": (i32, [vp, P(tfr_column), i32]),
         "tfr_batch_to_host": (i32, [vp, P(tfr_column), i32]),
@@ -254,6 +255,19 @@ class Batch:
         _check(lib().tfr_batch_dropped(self.h, C.byref(n), rec, off, code, field, k))
         return [(rec[i], off[i], code[i], field[i]) for i in range(k)]
 
+    def dropped_spans(self) -> List[tuple]:
+        """dropped() with each entry's byte length (tfr_batch_dropped_spans): 16 + L for a frame, p - o for a lost region
+        (TFR_F_RESYNC): [(entry index in the block, byte offset in the submitted buffer, byte length, TFR_E_* code, field)]"""
+        n = C.c_int64()
+        _check(lib().tfr_batch_dropped_spans(self.h, C.byref(n), None, None, None, None, None, 0))
+        k = n.value
+        if k == 0:
+            return []
+        rec, off, nb = (C.c_int64 * k)(), (C.c_int64 * k)(), (C.c_int64 * k)()
+        code, field = (C.c_int32 * k)(), (C.c_int32 * k)()
+        _check(lib().tfr_batch_dropped_spans(self.h, C.byref(n), rec, off, nb, code, field, k))
+        return [(rec[i], off[i], nb[i], code[i], field[i]) for i in range(k)]
+
     def to_host_async(self):
         """enqueue the D2H of every Arrow buffer behind the batch's kernels (overlaps the next batch)"""
         _check(lib().tfr_batch_to_host_async(self.h))
@@ -361,10 +375,11 @@ class Decoder:
         return lib().tfr_decoder_num_staging_slots()
 
     def stats(self) -> dict:
-        v = (C.c_int64 * 11)()
-        _check(lib().tfr_decoder_get_stats(self.h, v, 11))
+        v = (C.c_int64 * 13)()
+        _check(lib().tfr_decoder_get_stats(self.h, v, 13))
         names = ["batches", "speculative_submits", "speculative_redone", "count_mode_batches", "general_path_batches", "shapes_learned", "transcode_reruns",
                  "rows_async", "rows_async_rebuilt", "records_dropped", "records_corrupt"]
+        names += ["lost_regions", "lost_region_bytes"]                   # TFR_F_RESYNC
         return {k: v[i] for i, k in enumerate(names)}
 
     def stream(self) -> int:

@@ -25,6 +25,7 @@
 #include "host_util.h"
 #include "infer.cuh"
 #include "permissive.cuh"
+#include "resync.cuh"
 #include "rows.cuh"
 #include "scan.cuh"
 #include "tile.cuh"

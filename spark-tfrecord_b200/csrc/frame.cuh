@@ -88,6 +88,15 @@ __device__ __forceinline__ uint32_t frame_chain(const uint32_t* t0, const uint8_
   return q == nbytes ? FS_EOF : FS_LEFT;
 }
 
+// a plausible header at p (its 12 bytes inside the buffer): the upper half of the length is zero (the cheapest test, first),
+// the length fits an int32 and the stored CRC matches the masked CRC-32C of the 8 length bytes.  The candidate search below
+// and resync_scan_kernel (resync.cuh) look for record starts with it.
+__device__ __forceinline__ bool frame_header_ok(const uint32_t* t0, const uint8_t* data, uint32_t p) {
+  if (load_u32_unaligned(data + p + 4) != 0) return false;
+  const uint32_t lo = load_u32_unaligned(data + p);
+  return lo <= 0x7fffffffu && crc_mask(crc_u64(t0, lo, 0)) == load_u32_unaligned(data + p + 8);
+}
+
 // K1a -- candidate search, one WARP per chunk: 32 consecutive candidate offsets per step (coalesced: the warp's
 // loads fall into one or two sectors), cheapest condition first (the upper half of a plausible length is zero),
 // __ballot_sync picks the first hit.  The first 2 KiB of the chunk are prefetched by 16 lanes up front so the
@@ -117,11 +126,7 @@ __global__ void __launch_bounds__(256) frame_search_kernel(const uint8_t* __rest
         if (((p0 - cs) & 2047u) == 0 && lane < 17 && p0 + 128u * lane < nbytes)
           asm volatile("prefetch.global.L1 [%0];" ::"l"(data + p0 + 128u * lane));
         const uint32_t p = p0 + lane;
-        bool hit = false;
-        if (p <= last && load_u32_unaligned(data + p + 4) == 0) {
-          const uint32_t lo = load_u32_unaligned(data + p);
-          hit = lo <= 0x7fffffffu && crc_mask(crc_u64(t0, lo, 0)) == load_u32_unaligned(data + p + 8);
-        }
+        const bool hit = p <= last && frame_header_ok(t0, data, p);
         const uint32_t m = __ballot_sync(FULLMASK, hit);
         if (m) first = p0 + (uint32_t)(__ffs(m) - 1);
       }

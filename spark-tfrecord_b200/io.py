@@ -28,7 +28,7 @@ from typing import Dict, Iterator, List, Optional, Sequence
 import numpy as np
 
 from . import _cabi, _native
-from ._cabi import TFR_F_DEFAULT, TFR_F_DROP_MALFORMED, TFR_F_PERMISSIVE, TFR_E_BATCH_TOO_LARGE as A_TFR_E_BATCH_TOO_LARGE, columns_from_rows
+from ._cabi import TFR_F_DEFAULT, TFR_F_DROP_MALFORMED, TFR_F_PERMISSIVE, TFR_F_RESYNC, TFR_E_BATCH_TOO_LARGE as A_TFR_E_BATCH_TOO_LARGE, columns_from_rows
 from .sqltypes import RECORD_TYPES, BinaryType, StructField, StructType, byte_array_schema
 
 M = "src/main/scala/com/linkedin/spark/datasources/tfrecord/"
@@ -57,17 +57,34 @@ def _parse_mode(options: Optional[Dict[str, str]]) -> str:
                                                f"PERMISSIVE with a corrupt-record column")
 
 
+def _resync_flag(options: Optional[Dict[str, str]], mode: str) -> int:
+    """the `resyncFraming` option ("false" by default, or "true", case-insensitive) -> 0 or TFR_F_RESYNC: after a framing
+    error (a bad length CRC, a length above 2^31 - 1, a record cut off at the end of the file) reading goes on at the next
+    record whose two CRCs verify, instead of failing the file.  DROPMALFORMED drops the bytes in between, PERMISSIVE reads
+    them as one corrupt row.  Only with those two modes: FAILFAST is the reference's behaviour and stays so."""
+    value = (options or {}).get("resyncFraming", "false")
+    v = value.lower() if isinstance(value, str) else value
+    if v not in ("true", "false"):
+        raise _native.IllegalArgumentException(-1, f"resyncFraming {value}: the option takes true or false")
+    if v == "false":
+        return 0
+    if mode not in ("DROPMALFORMED", "PERMISSIVE"):
+        raise _native.IllegalArgumentException(-1, f"resyncFraming needs mode DROPMALFORMED or PERMISSIVE (mode {mode})")
+    return TFR_F_RESYNC
+
+
 def _decoder_flags(options: Optional[Dict[str, str]], dataSchema: Optional[StructType] = None) -> int:
     """the `mode` option -> decoder flags.  FAILFAST (the default, the reference's behaviour): the first failing record
     ends the file.  DROPMALFORMED: failing records are dropped and the rest is read (framing errors still end the file).
     PERMISSIVE: a failing record is read as a row of nulls; it needs a corrupt-record column in `dataSchema` (a field
     named by columnNameOfCorruptRecord, nullable BinaryType), which receives the record's payload, and Example or
-    SequenceExample records."""
+    SequenceExample records.  resyncFraming=true (DROPMALFORMED and PERMISSIVE only) adds TFR_F_RESYNC."""
     m = _parse_mode(options)
+    resync = _resync_flag(options, m)
     if m == "FAILFAST":
         return TFR_F_DEFAULT
     if m == "DROPMALFORMED":
-        return TFR_F_DEFAULT | TFR_F_DROP_MALFORMED
+        return TFR_F_DEFAULT | TFR_F_DROP_MALFORMED | resync
     if m == "PERMISSIVE":
         name = _corrupt_column_name(options)
         field = next((f for f in dataSchema or () if f.name == name), None)
@@ -80,7 +97,7 @@ def _decoder_flags(options: Optional[Dict[str, str]], dataSchema: Optional[Struc
         if _record_type(options) == RECORD_TYPES["ByteArray"]:
             raise _native.IllegalArgumentException(-1, "mode PERMISSIVE: ByteArray records have no corrupt-record column; "
                                                        "use FAILFAST or DROPMALFORMED")
-        return TFR_F_DEFAULT | TFR_F_PERMISSIVE
+        return TFR_F_DEFAULT | TFR_F_PERMISSIVE | resync
 
 
 def _read_mode(options: Optional[Dict[str, str]], dataSchema: StructType, requiredSchema: StructType):
@@ -315,7 +332,9 @@ class TFRecordFileReader:
         handed out.  Rows before a bad record are yielded, then the exception the reference would throw is raised.
         With options["mode"] = "DROPMALFORMED" a failing record is skipped instead (a framing error still raises), and
         the dropped records of each block are logged once, with the file offset of the first.  With "PERMISSIVE" it is a
-        row of nulls, its payload in the corrupt-record column when `schema` holds it, and logged the same way.
+        row of nulls, its payload in the corrupt-record column when `schema` holds it, and logged the same way.  With
+        resyncFraming = "true" as well, a framing error does not raise: the bytes up to the next verified record are a lost
+        region, dropped or read as one corrupt row, and each is logged with its file offset and length.
         `dataSchema` (default: `schema`) is the file's schema, which PERMISSIVE needs the corrupt-record column in."""
         rt = _record_type(options)
         flags, corrupt = _read_mode(options, schema if dataSchema is None else dataSchema, schema)
@@ -352,6 +371,14 @@ class TFRecordFileReader:
                                 yield row
                             if flags & (TFR_F_DROP_MALFORMED | TFR_F_PERMISSIVE):
                                 dropped = batch.dropped()
+                                if flags & TFR_F_RESYNC:
+                                    for _, off, nb, code, _ in batch.dropped_spans():
+                                        if code in _cabi.FRAMING_ERRORS:
+                                            _LOG.warning("%s: %s %d bytes at file offset %d (%s); reading goes on at the next "
+                                                         "verified record", file.toPath(),
+                                                         "read as a corrupt row" if flags & TFR_F_PERMISSIVE else "lost", nb,
+                                                         block_pos + off, _cabi.STATUS_NAMES.get(code, code))
+                                    dropped = [e for e in dropped if e[2] not in _cabi.FRAMING_ERRORS]
                                 if dropped:
                                     _LOG.warning("%s: %s %d malformed record(s) of the block at offset %d; the first at "
                                                  "file offset %d (%s)", file.toPath(),
@@ -446,18 +473,21 @@ class DefaultSource:
         ByteArray has the fixed one-column schema.  With `dist`, every rank scans its shard of the files and the maps
         are merged with one all-reduce (sharding.allreduce_schema).
         options["mode"] as the reader takes it: FAILFAST (default) fails on the first failing record.  DROPMALFORMED and
-        PERMISSIVE skip failing records (framing errors still fail), logging them once per file, and without `dist` take
+        PERMISSIVE skip failing records (framing errors still fail, unless resyncFraming is "true": then the bytes up to
+        the next verified record are skipped, each such region logged with its file offset), logging them once per file, and without `dist` take
         the first file whose records give any name (the reference's collectFirst(hasSchema), M/DefaultSource.scala:36-38),
         since a file of skipped records only would give an empty schema.  PERMISSIVE ignores features named by
         columnNameOfCorruptRecord and always ends the schema with that column (nullable BinaryType), so that the schema
         reads the files back under the options it was inferred with (buildReader refuses PERMISSIVE without it)."""
         from .sharding import allreduce_schema, codes_to_struct, shard_lpt
         mode = _parse_mode(options)
+        resync = _resync_flag(options, mode)
         rt = _record_type(options)
         if rt == 2:
             return byte_array_schema()
         corrupt = _corrupt_column_name(options) if mode == "PERMISSIVE" else None
         flags = {"FAILFAST": 0, "DROPMALFORMED": TFR_F_DEFAULT | TFR_F_DROP_MALFORMED, "PERMISSIVE": TFR_F_DEFAULT | TFR_F_PERMISSIVE}[mode]
+        flags |= resync
         distributed = dist is not None and dist.is_initialized()
         todo = [f for f in files if os.path.getsize(f) > 0]
         if distributed:
@@ -488,6 +518,12 @@ class DefaultSource:
                     remaining = (1 << 62) if _codec_of_path(f) is not None else os.path.getsize(f)
                     for _ in _stream_blocks(fh, remaining, block, stage, process):
                         pass
+                if flags & TFR_F_RESYNC:
+                    for off, code in skipped:
+                        if code in _cabi.FRAMING_ERRORS:
+                            _LOG.warning("%s: schema inference skipped the bytes from file offset %d to the next verified record (%s)",
+                                         f, off, _cabi.STATUS_NAMES.get(code, code))
+                    skipped = [e for e in skipped if e[1] not in _cabi.FRAMING_ERRORS]
                 if skipped:
                     _LOG.warning("%s: schema inference skipped %d malformed record(s); the first at file offset %d (%s)", f,
                                  len(skipped), skipped[0][0], _cabi.STATUS_NAMES.get(skipped[0][1], skipped[0][1]))

@@ -18,6 +18,7 @@
 //     static native java.nio.ByteBuffer[] batchColumnHost(long batch, int column, long[] meta);  // validity, offsets*, values
 //     static native void batchExportArrowDevice(long batch, int column, long arrowDeviceArrayAddr, long arrowSchemaAddr);  // ColumnarBatch on the GPU (spark-rapids)
 //     static native long[] batchDropped(long batch, int maxEntries);   // {nDropped, (record, offset, code, field)*}: DROPMALFORMED, PERMISSIVE
+//     static native long[] batchDroppedSpans(long batch, int maxEntries);   // {nDropped, (record, offset, nbytes, code, field)*}: + lost regions (resyncFraming)
 //     static native void batchThrowIfError(long batch);   // the exception the reference would throw for the first failing record
 //     static native void batchRelease(long batch);
 //     static native java.nio.ByteBuffer[] batchRows(long batch);   // {rows, int64 row offsets}: pinned UnsafeRows, valid until batchRelease
@@ -160,6 +161,24 @@ extern "C" JNIEXPORT jlongArray JNICALL Java_com_linkedin_spark_datasources_tfre
   std::vector<jlong> v(1 + 4 * k);
   v[0] = (jlong)n;
   for (int64_t i = 0; i < k; ++i) { v[1 + 4 * i] = rec[i]; v[2 + 4 * i] = off[i]; v[3 + 4 * i] = code[i]; v[4 + 4 * i] = field[i]; }
+  jlongArray a = env->NewLongArray((jsize)v.size()); env->SetLongArrayRegion(a, 0, (jsize)v.size(), v.data());
+  return a;
+}
+// batchDropped with each entry's byte length: 16 + L for a frame, the region's length for a lost region (decoder flag
+// TFR_F_RESYNC, option resyncFraming).  The reader logs each lost region once, at block offset + offset, with its length.
+extern "C" JNIEXPORT jlongArray JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_batchDroppedSpans(JNIEnv* env, jclass, jlong batch, jint maxEntries) {
+  int64_t n = 0;
+  int32_t rc = tfr_batch_dropped_spans((tfr_batch*)batch, &n, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
+  if (rc) { tfr_batch_release((tfr_batch*)batch); throw_for(env, rc, -1); return nullptr; }
+  const int64_t k = maxEntries < 0 ? 0 : (n < maxEntries ? n : (int64_t)maxEntries);
+  std::vector<int64_t> rec(k), off(k), nb(k);
+  std::vector<int32_t> code(k), field(k);
+  if (k) tfr_batch_dropped_spans((tfr_batch*)batch, &n, rec.data(), off.data(), nb.data(), code.data(), field.data(), k);
+  std::vector<jlong> v(1 + 5 * k);
+  v[0] = (jlong)n;
+  for (int64_t i = 0; i < k; ++i) {
+    v[1 + 5 * i] = rec[i]; v[2 + 5 * i] = off[i]; v[3 + 5 * i] = nb[i]; v[4 + 5 * i] = code[i]; v[5 + 5 * i] = field[i];
+  }
   jlongArray a = env->NewLongArray((jsize)v.size()); env->SetLongArrayRegion(a, 0, (jsize)v.size(), v.data());
   return a;
 }
