@@ -245,15 +245,7 @@ class Batch:
         """the records a drop-mode decoder (TFR_F_DROP_MALFORMED) cut out of this batch, or a PERMISSIVE one delivered as
         corrupt rows, in record order (tfr_batch_dropped):
         [(frame index in the block, byte offset in the submitted buffer, TFR_E_* code, schema field or -1)]"""
-        n = C.c_int64()
-        _check(lib().tfr_batch_dropped(self.h, C.byref(n), None, None, None, None, 0))
-        k = n.value
-        if k == 0:
-            return []
-        rec, off = (C.c_int64 * k)(), (C.c_int64 * k)()
-        code, field = (C.c_int32 * k)(), (C.c_int32 * k)()
-        _check(lib().tfr_batch_dropped(self.h, C.byref(n), rec, off, code, field, k))
-        return [(rec[i], off[i], code[i], field[i]) for i in range(k)]
+        return [(rec, off, code, field) for rec, off, _, code, field in self.dropped_spans()]
 
     def dropped_spans(self) -> List[tuple]:
         """dropped() with each entry's byte length (tfr_batch_dropped_spans): 16 + L for a frame, p - o for a lost region

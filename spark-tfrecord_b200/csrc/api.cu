@@ -358,6 +358,8 @@ static cudaError_t raise_dyn_smem(size_t smem) {
   return e;
 }
 
+#include "api_frames.inc"
+#include "api_infer.inc"
 #include "api_decode.inc"
 #include "api_rows.inc"
 

@@ -347,5 +347,9 @@ __host__ __device__ __forceinline__ int type_width(int t) {
   }
 }
 
-// per-record status word: code in the low 8 bits (negated TFR_E_*), field index + 1 above
+// per-record status word: code in the low 8 bits (negated TFR_E_*), field index + 1 above; the top bit is DF_REGION
 __device__ __forceinline__ uint32_t make_status(int code, int field) { return (uint32_t)(-code) | ((uint32_t)(field + 1) << 8); }
+// the status of a lost region (TFR_F_RESYNC) in a failing-record list: its code is the framing error, its field -1
+#define DF_REGION 0x80000000u
+__host__ __device__ __forceinline__ int32_t status_code(uint32_t s) { return -(int32_t)(s & 0xff); }
+__host__ __device__ __forceinline__ int32_t status_field(uint32_t s) { return (int32_t)((s & ~DF_REGION) >> 8) - 1; }

@@ -8,8 +8,8 @@
 #pragma once
 #include "common.cuh"
 
-// one dropped record: its frame index in the batch, its frame [off, end) in the batch's bytes, its pass-1 status
-// ((TFR_E_* negated) | (schema field + 1) << 8)
+// one dropped record: its frame index in the batch, its frame [off, end) in the batch's bytes, its pass-1 status (the status
+// word of common.cuh: make_status, status_code, status_field, DF_REGION)
 struct DroppedFrame { uint32_t row, off, end, status; };
 static_assert(sizeof(DroppedFrame) == 16, "DroppedFrame layout");
 

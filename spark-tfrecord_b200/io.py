@@ -23,7 +23,7 @@ from __future__ import annotations
 import logging
 import os
 import struct
-from typing import Dict, Iterator, List, Optional, Sequence
+from typing import Dict, Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -73,18 +73,22 @@ def _resync_flag(options: Optional[Dict[str, str]], mode: str) -> int:
     return TFR_F_RESYNC
 
 
+_MODE_FLAGS = {"FAILFAST": TFR_F_DEFAULT, "DROPMALFORMED": TFR_F_DEFAULT | TFR_F_DROP_MALFORMED, "PERMISSIVE": TFR_F_DEFAULT | TFR_F_PERMISSIVE}
+
+
+def _mode_flags(options: Optional[Dict[str, str]]) -> Tuple[str, int]:
+    """the `mode` and `resyncFraming` options -> (mode, flags of the decoder and of schema inference)"""
+    m = _parse_mode(options)
+    return m, _MODE_FLAGS[m] | _resync_flag(options, m)
+
+
 def _decoder_flags(options: Optional[Dict[str, str]], dataSchema: Optional[StructType] = None) -> int:
     """the `mode` option -> decoder flags.  FAILFAST (the default, the reference's behaviour): the first failing record
     ends the file.  DROPMALFORMED: failing records are dropped and the rest is read (framing errors still end the file).
     PERMISSIVE: a failing record is read as a row of nulls; it needs a corrupt-record column in `dataSchema` (a field
     named by columnNameOfCorruptRecord, nullable BinaryType), which receives the record's payload, and Example or
     SequenceExample records.  resyncFraming=true (DROPMALFORMED and PERMISSIVE only) adds TFR_F_RESYNC."""
-    m = _parse_mode(options)
-    resync = _resync_flag(options, m)
-    if m == "FAILFAST":
-        return TFR_F_DEFAULT
-    if m == "DROPMALFORMED":
-        return TFR_F_DEFAULT | TFR_F_DROP_MALFORMED | resync
+    m, flags = _mode_flags(options)
     if m == "PERMISSIVE":
         name = _corrupt_column_name(options)
         field = next((f for f in dataSchema or () if f.name == name), None)
@@ -97,7 +101,7 @@ def _decoder_flags(options: Optional[Dict[str, str]], dataSchema: Optional[Struc
         if _record_type(options) == RECORD_TYPES["ByteArray"]:
             raise _native.IllegalArgumentException(-1, "mode PERMISSIVE: ByteArray records have no corrupt-record column; "
                                                        "use FAILFAST or DROPMALFORMED")
-        return TFR_F_DEFAULT | TFR_F_PERMISSIVE | resync
+    return flags
 
 
 def _read_mode(options: Optional[Dict[str, str]], dataSchema: StructType, requiredSchema: StructType):
@@ -480,14 +484,11 @@ class DefaultSource:
         columnNameOfCorruptRecord and always ends the schema with that column (nullable BinaryType), so that the schema
         reads the files back under the options it was inferred with (buildReader refuses PERMISSIVE without it)."""
         from .sharding import allreduce_schema, codes_to_struct, shard_lpt
-        mode = _parse_mode(options)
-        resync = _resync_flag(options, mode)
+        mode, flags = _mode_flags(options)
         rt = _record_type(options)
         if rt == 2:
             return byte_array_schema()
         corrupt = _corrupt_column_name(options) if mode == "PERMISSIVE" else None
-        flags = {"FAILFAST": 0, "DROPMALFORMED": TFR_F_DEFAULT | TFR_F_DROP_MALFORMED, "PERMISSIVE": TFR_F_DEFAULT | TFR_F_PERMISSIVE}[mode]
-        flags |= resync
         distributed = dist is not None and dist.is_initialized()
         todo = [f for f in files if os.path.getsize(f) > 0]
         if distributed:
