@@ -360,6 +360,7 @@ static cudaError_t raise_dyn_smem(size_t smem) {
 
 #include "api_frames.inc"
 #include "api_infer.inc"
+#include "api_outputs.inc"
 #include "api_decode.inc"
 #include "api_rows.inc"
 
@@ -435,8 +436,8 @@ static void build_array(ArrowArray* a, const tfr_column& c, int level, int64_t l
 }
 
 extern "C" int32_t tfr_batch_export_arrow_host(tfr_batch* b, int32_t column, void* arrow_array, void* arrow_schema) {
-  if (!b || !arrow_array || !arrow_schema || column < 0 || column >= (int32_t)b->cols.size()) return fail(TFR_E_INVALID_ARG, "bad argument");
-  int32_t rc = tfr_batch_to_host(b, nullptr, (int32_t)b->cols.size());
+  if (!b || !arrow_array || !arrow_schema || column < 0 || column >= (int32_t)b->out.cols.size()) return fail(TFR_E_INVALID_ARG, "bad argument");
+  int32_t rc = tfr_batch_to_host(b, nullptr, (int32_t)b->out.cols.size());
   if (rc) return rc;
   const tfr_column& c = b->host_copy.cols[column];
   const tfr_schema& S = b->dec->schema;
@@ -446,10 +447,10 @@ extern "C" int32_t tfr_batch_export_arrow_host(tfr_batch* b, int32_t column, voi
   return TFR_OK;
 }
 extern "C" int32_t tfr_batch_export_arrow_device(tfr_batch* b, int32_t column, void* arrow_device_array, void* arrow_schema) {
-  if (!b || !arrow_device_array || !arrow_schema || column < 0 || column >= (int32_t)b->cols.size()) return fail(TFR_E_INVALID_ARG, "bad argument");
+  if (!b || !arrow_device_array || !arrow_schema || column < 0 || column >= (int32_t)b->out.cols.size()) return fail(TFR_E_INVALID_ARG, "bad argument");
   int32_t rc = tfr_batch_wait(b);
   if (rc) return rc;
-  const tfr_column& c = b->cols[column];
+  const tfr_column& c = b->out.cols[column];
   const tfr_schema& S = b->dec->schema;
   std::string nm((const char*)&S.names[S.fields[column].name_off], S.fields[column].name_len);
   build_schema((ArrowSchema*)arrow_schema, nm.c_str(), c.elem_type, c.depth);
