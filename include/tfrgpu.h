@@ -63,7 +63,13 @@ enum {
   TFR_T_FLOAT64 = 4,  /* DoubleType <- FloatList widened (:83-84); written via toFloat        */
   TFR_T_DECIMAL = 5,  /* DecimalType: carried as float64 (f.toDouble, :86-87); the JVM shim wraps it in Decimal */
   TFR_T_STRING  = 6,  /* StringType <- BytesList, Java UTF-8 decode/re-encode semantics (:89-91) */
-  TFR_T_BINARY  = 7   /* BinaryType <- BytesList raw (:93-95)                                 */
+  TFR_T_BINARY  = 7,  /* BinaryType <- BytesList raw (:93-95)                                 */
+  /* Generated fields: metadata of the row, never read from a record (POSITIONS below).  Decoder schemas only: at depth 0,
+   * at most one of each kind, or tfr_schema_create returns TFR_E_UNSUPPORTED_TYPE naming the field; tfr_encoder_create
+   * refuses a schema that has one (TFR_E_UNSUPPORTED_TYPE).  Their tfr_column reports TFR_T_INT64, depth 0, null_count 0
+   * and every validity bit set, so every view of a batch (columns, host copy, Arrow, UnsafeRows) reads them as LongType. */
+  TFR_T_ROW_INDEX     = 8,  /* the row's entry index in its file                                */
+  TFR_T_RECORD_OFFSET = 9   /* the file offset of the row's entry                               */
 };
 
 /* record types: the `recordType` DataSource option (M/TFRecordFileReader.scala:22,69-80) */
@@ -92,7 +98,9 @@ const char* tfr_last_error(void);
 
 /* Replaces `new TFRecordDeserializer(schema)` (M/TFRecordFileReader.scala:44) and
  * `new TFRecordSerializer(dataSchema)` (M/TFRecordOutputWriter.scala:24): validates the types
- * up front the way TFRecordSerializer's constructor does (M/TFRecordSerializer.scala:14).   */
+ * up front the way TFRecordSerializer's constructor does (M/TFRecordSerializer.scala:14).
+ * TFR_RT_BYTE_ARRAY: the one field `byteArray`, then the generated fields of `fields` in their order; the other fields of
+ * `fields` are ignored.                                                                                              */
 int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, int32_t record_type,
                           tfr_schema** out);
 void    tfr_schema_destroy(tfr_schema*);
@@ -155,6 +163,25 @@ int32_t tfr_schema_num_fields(const tfr_schema*);
  * lost regions ([11]) and their bytes ([12]); counters [9] and [10] count records only.                                  */
 #define TFR_F_RESYNC       0x8u
 #define TFR_F_DEFAULT      (TFR_F_VERIFY_CRC)
+/* POSITIONS: the generated fields TFR_T_ROW_INDEX and TFR_T_RECORD_OFFSET (Spark's `_metadata.row_index`).  A batch's
+ * ENTRIES are its frames and its lost regions (TFR_F_RESYNC) in byte order: what n_records counts and what
+ * tfr_batch_dropped's `record` indexes.  Within one file:
+ *   - row index     = the row's entry index in the file, counted from 0 at the file's first byte.  Every frame counts:
+ *                     dropped ones, corrupt ones, and the frames of a FAILFAST block before its error.  A lost region
+ *                     counts as one entry.
+ *   - record offset = the file offset of the entry's first byte: the frame's 12-byte header, or `o` for a lost region.  For
+ *                     a compressed file it is an offset in the decompressed stream.
+ *   - Both are int64 and non-null on every delivered row, PERMISSIVE's corrupt rows included: they are metadata, not data
+ *     fields, so PERMISSIVE's "every data field null" does not apply to them.
+ *   - A record feature named like a generated field is never looked up (it is still validated, like any feature outside
+ *     the schema), as for the corrupt-record column.
+ * A block knows its position in the file from tfr_decode_at / tfr_decode_submit_at (first_entry, first_offset: the file
+ * position of its first byte); a streaming reader carries them from block to block with tfr_batch_extent.  So:
+ *   - FAILFAST without errors: row r of a block has row index first_entry + r;
+ *   - DROPMALFORMED: row indexes rise strictly and skip exactly the dropped entries;
+ *   - PERMISSIVE: a corrupt row has (row index, record offset) = (first_entry + its tfr_batch_dropped record,
+ *     first_offset + its tfr_batch_dropped offset);
+ *   - in every mode the values do not depend on where the blocks are cut.                                               */
 
 /* Replaces TFRecordFileReader.readFile's setup (M/TFRecordFileReader.scala:16-44):
  * binds a device, a CUDA stream and reusable device/pinned buffers.                        */
@@ -205,6 +232,13 @@ int32_t tfr_decode(tfr_decoder*, const void* data, size_t nbytes, int32_t data_o
                    int32_t is_final, tfr_batch** out, size_t* consumed);
 int32_t tfr_decode_submit(tfr_decoder*, const void* data, size_t nbytes, int32_t data_on_device,
                           int32_t is_final, tfr_batch** out);
+/* The same calls for a block whose first byte is entry `first_entry` at offset `first_offset` of its file (POSITIONS
+ * above): the base of the generated fields.  tfr_decode and tfr_decode_submit are these with (0, 0).  A negative value is
+ * TFR_E_INVALID_ARG, before any device work.  Every redo of the batch keeps its base.                                  */
+int32_t tfr_decode_at(tfr_decoder*, const void* data, size_t nbytes, int32_t data_on_device, int32_t is_final,
+                      int64_t first_entry, int64_t first_offset, tfr_batch** out, size_t* consumed);
+int32_t tfr_decode_submit_at(tfr_decoder*, const void* data, size_t nbytes, int32_t data_on_device, int32_t is_final,
+                             int64_t first_entry, int64_t first_offset, tfr_batch** out);
 
 int32_t tfr_decoder_stream(tfr_decoder*, void** cuda_stream /* cudaStream_t */);
 
@@ -251,6 +285,10 @@ int32_t tfr_batch_status(tfr_batch*, tfr_batch_info* out);
  * index of block t+1.  For a batch that later reports an error, tfr_batch_info.consumed_bytes (the bytes in front of the
  * failing record) is what counts; the reader stops there anyway.                                                     */
 int32_t tfr_batch_consumed(tfr_batch*, size_t* consumed);
+/* tfr_batch_consumed plus the entries in the consumed bytes (POSITIONS above), with the same wait: a streaming reader passes
+ * first_entry += *entries and first_offset += *consumed to its next submit.  Under TFR_F_RESYNC a framing stop resolves the
+ * batch here, as in tfr_batch_consumed.  Either output may be NULL.                                                     */
+int32_t tfr_batch_extent(tfr_batch*, size_t* consumed, int64_t* entries);
 /* The records a TFR_F_DROP_MALFORMED decoder dropped from this batch.  Waits for and resolves the batch like
  * tfr_batch_status, sets *n_dropped to their number and fills the first min(*n_dropped, cap) entries, in record order:
  * the frame index within the block, the frame's byte offset in the submitted buffer (a reader adds the block's file

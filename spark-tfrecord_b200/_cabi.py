@@ -9,7 +9,7 @@ from typing import List, Sequence
 import numpy as np
 
 from .sqltypes import (StructType, lower_type, TFR_T_NULL, TFR_T_INT32, TFR_T_INT64, TFR_T_FLOAT32,
-                       TFR_T_FLOAT64, TFR_T_DECIMAL, TFR_T_STRING, TFR_T_BINARY)
+                       TFR_T_FLOAT64, TFR_T_DECIMAL, TFR_T_STRING, TFR_T_BINARY, TFR_T_ROW_INDEX, TFR_T_RECORD_OFFSET)
 
 TFR_OK = 0
 TFR_E_INVALID_ARG = -1

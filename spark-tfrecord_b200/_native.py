@@ -22,7 +22,7 @@ _LIB = None
 EXPORTS = [
     "tfr_abi_version", "tfr_status_string", "tfr_last_error", "tfr_schema_create", "tfr_schema_destroy",
     "tfr_schema_num_fields", "tfr_decoder_create", "tfr_decoder_create_permissive", "tfr_decoder_destroy", "tfr_decoder_staging", "tfr_decoder_staging_slot",
-    "tfr_decoder_num_staging_slots", "tfr_decode", "tfr_decode_submit",
+    "tfr_decoder_num_staging_slots", "tfr_decode", "tfr_decode_submit", "tfr_decode_at", "tfr_decode_submit_at", "tfr_batch_extent",
     "tfr_decoder_stream", "tfr_decoder_set_profiling", "tfr_decoder_get_profile", "tfr_decoder_get_stats", "tfr_batch_wait", "tfr_batch_status", "tfr_batch_consumed", "tfr_batch_dropped", "tfr_batch_dropped_spans", "tfr_batch_num_columns", "tfr_batch_columns",
     "tfr_batch_to_host_async", "tfr_batch_to_host", "tfr_batch_export_arrow_host", "tfr_batch_export_arrow_device", "tfr_batch_release",
     "tfr_batch_rows", "tfr_batch_rows_with_partition", "tfr_batch_rows_async",
@@ -113,6 +113,9 @@ def lib():
         "tfr_decoder_num_staging_slots": (i32, []),
         "tfr_decode": (i32, [vp, vp, sz, i32, i32, P(vp), P(sz)]),
         "tfr_decode_submit": (i32, [vp, vp, sz, i32, i32, P(vp)]),
+        "tfr_decode_at": (i32, [vp, vp, sz, i32, i32, i64, i64, P(vp), P(sz)]),
+        "tfr_decode_submit_at": (i32, [vp, vp, sz, i32, i32, i64, i64, P(vp)]),
+        "tfr_batch_extent": (i32, [vp, P(C.c_size_t), P(i64)]),
         "tfr_decoder_get_stats": (i32, [vp, P(i64), i32]),
         "tfr_batch_to_host_async": (i32, [vp]),
         "tfr_infer_update_block": (i32, [vp, vp, sz, i32, i32, P(sz)]),
@@ -241,6 +244,13 @@ class Batch:
         _check(lib().tfr_batch_consumed(self.h, C.byref(n)))
         return n.value
 
+    def extent(self) -> tuple:
+        """(consumed bytes, entries in them) with consumed()'s wait (tfr_batch_extent): a streaming reader adds them to the
+        next block's first_offset and first_entry"""
+        n, e = C.c_size_t(), C.c_int64()
+        _check(lib().tfr_batch_extent(self.h, C.byref(n), C.byref(e)))
+        return n.value, e.value
+
     def dropped(self) -> List[tuple]:
         """the records a drop-mode decoder (TFR_F_DROP_MALFORMED) cut out of this batch, or a PERMISSIVE one delivered as
         corrupt rows, in record order (tfr_batch_dropped):
@@ -342,7 +352,7 @@ class Decoder:
         """`corrupt_field`: with TFR_F_PERMISSIVE in `flags`, the index of the schema field that receives a failing record's
         payload (a nullable BinaryType column; tfr_decoder_create_permissive)"""
         self.schema = Schema(schema, record_type)
-        self.ncols = 1 if record_type == 2 else len(schema)
+        self.ncols = lib().tfr_schema_num_fields(self.schema.h)     # ByteArray: byteArray, then the generated fields
         h = C.c_void_p()
         if corrupt_field is None:
             _check(lib().tfr_decoder_create(self.schema.h, device, flags, C.byref(h)))
@@ -390,23 +400,25 @@ class Decoder:
         names = ["frame_index", "pass1", "scan", "pass2", "pack_validity", "h2d", "d2h", "rows"]
         return {"ms": {k: ms[i] for i, k in enumerate(names)}, "launches": nl.value, "pass1_launches": n1.value}
 
-    def decode(self, data, is_final: bool = True, nbytes: Optional[int] = None):
-        """-> (Batch, consumed_bytes)"""
+    def decode(self, data, is_final: bool = True, nbytes: Optional[int] = None, first_entry: int = 0, first_offset: int = 0):
+        """-> (Batch, consumed_bytes).  first_entry / first_offset: the block's position in its file, the base of the
+        generated fields (tfr_decode_at)"""
         ptr, n, on_dev, keep = _device_ptr(data)
         if nbytes is not None:
             n = nbytes
         b = C.c_void_p()
         used = C.c_size_t()
-        _check(lib().tfr_decode(self.h, ptr, n, on_dev, 1 if is_final else 0, C.byref(b), C.byref(used)))
+        _check(lib().tfr_decode_at(self.h, ptr, n, on_dev, 1 if is_final else 0, first_entry, first_offset, C.byref(b), C.byref(used)))
         return Batch(b, self.ncols), used.value
 
-    def submit(self, data, is_final: bool = True, nbytes: Optional[int] = None) -> "Batch":
-        """pipelined decode (tfr_decode_submit): returns at once; Batch.info["consumed_bytes"] has the consumed count"""
+    def submit(self, data, is_final: bool = True, nbytes: Optional[int] = None, first_entry: int = 0,
+               first_offset: int = 0) -> "Batch":
+        """pipelined decode (tfr_decode_submit_at): returns at once; Batch.info["consumed_bytes"] has the consumed count"""
         ptr, n, on_dev, keep = _device_ptr(data)
         if nbytes is not None:
             n = nbytes
         b = C.c_void_p()
-        _check(lib().tfr_decode_submit(self.h, ptr, n, on_dev, 1 if is_final else 0, C.byref(b)))
+        _check(lib().tfr_decode_submit_at(self.h, ptr, n, on_dev, 1 if is_final else 0, first_entry, first_offset, C.byref(b)))
         return Batch(b, self.ncols, keep)
 
     def close(self):

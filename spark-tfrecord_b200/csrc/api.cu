@@ -25,6 +25,7 @@
 #include "host_util.h"
 #include "infer.cuh"
 #include "permissive.cuh"
+#include "position.cuh"
 #include "resync.cuh"
 #include "rows.cuh"
 #include "scan.cuh"
@@ -188,9 +189,36 @@ struct tfr_schema {
   std::vector<int32_t> var_field;    // var slot -> field
   std::vector<int32_t> fix_field;    // fix slot -> field
   int32_t n_fix = 0, n_var = 0, n_cnt = 0;
+  // the generated fields (TFR_T_ROW_INDEX, TFR_T_RECORD_OFFSET): their field, -1 none.  Lowered to nullable int64 columns that
+  // are left out of the key hash table; position_kernel fills them.
+  int32_t gen_field[2] = {-1, -1};
+  bool generated(int32_t f) const { return f >= 0 && (f == gen_field[0] || f == gen_field[1]); }
+  bool has_generated() const { return gen_field[0] >= 0 || gen_field[1] >= 0; }
 };
 
 static uint32_t fnv1a(const uint8_t* p, uint32_t n) { uint32_t h = 2166136261u; for (uint32_t i = 0; i < n; ++i) h = (h ^ p[i]) * 16777619u; return h; }
+
+// A generated field of `f` (TFR_T_ROW_INDEX, TFR_T_RECORD_OFFSET) appended to `s` as a nullable int64 column; false when f is
+// not one.  Anything but depth 0 and one field of each kind is TFR_E_UNSUPPORTED_TYPE in *rc.
+static bool add_generated(tfr_schema& s, const tfr_field& f, const std::string& nm, int32_t* rc) {
+  if (f.elem_type != TFR_T_ROW_INDEX && f.elem_type != TFR_T_RECORD_OFFSET) return false;
+  const int kind = f.elem_type - TFR_T_ROW_INDEX;
+  if (f.depth != 0) { *rc = fail(TFR_E_UNSUPPORTED_TYPE, "field '" + nm + "': a generated field is a scalar (depth 0)"); return true; }
+  if (s.gen_field[kind] >= 0) { *rc = fail(TFR_E_UNSUPPORTED_TYPE, "field '" + nm + "': a schema has at most one generated field of each kind"); return true; }
+  DevField d{};
+  d.name_off = (uint32_t)s.names.size(); d.name_len = (uint32_t)f.name_len;
+  s.names.insert(s.names.end(), (const uint8_t*)f.name, (const uint8_t*)f.name + f.name_len);
+  d.hash = fnv1a((const uint8_t*)f.name, d.name_len);
+  d.elem_type = TFR_T_INT64; d.depth = 0; d.nullable = 1; d.kind = (int8_t)required_kind(TFR_T_INT64); d.n_levels = 0; d.dup_next = -1;
+  d.width = 8; d.var_slot = -1; d.cnt_slot = -1;
+  d.fix_slot = s.n_fix++; s.fix_field.push_back((int32_t)s.fields.size());
+  s.gen_field[kind] = (int32_t)s.fields.size();
+  s.fields.push_back(d);
+  *rc = TFR_OK;
+  return true;
+}
+
+static void schema_rehash(tfr_schema& s, int32_t skip);
 
 extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, int32_t record_type, tfr_schema** out) {
   if (!out || n_fields < 0 || (n_fields > 0 && !fields)) return fail(TFR_E_INVALID_ARG, "null argument");
@@ -201,7 +229,7 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
   s->record_type = record_type;
   if (record_type == TFR_RT_BYTE_ARRAY) {
     // the single binary column of TensorFlowInferSchema.getSchemaForByteArray (M/TensorFlowInferSchema.scala:60-64);
-    // the caller's field list is ignored like deserializeByteArray ignores the schema (:17-19)
+    // the caller's field list is ignored like deserializeByteArray ignores the schema (:17-19), but for generated fields
     DevField d{};
     d.name_off = 0; d.name_len = 9; s->names.assign((const uint8_t*)"byteArray", (const uint8_t*)"byteArray" + 9);
     d.hash = fnv1a(s->names.data(), 9);
@@ -212,6 +240,14 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
     s->n_var = 1; s->n_cnt = 1;
     s->ht.assign(2, -1);
     s->ht[d.hash & 1] = 0;
+    for (int32_t i = 0; i < n_fields; ++i) {
+      const tfr_field& f = fields[i];
+      if (f.elem_type != TFR_T_ROW_INDEX && f.elem_type != TFR_T_RECORD_OFFSET) continue;
+      if (f.name_len < 0 || (f.name_len > 0 && !f.name)) return fail(TFR_E_INVALID_ARG, "bad field name");
+      int32_t rc = TFR_OK;
+      add_generated(*s, f, std::string(f.name ? f.name : "", (size_t)f.name_len), &rc);
+      if (rc) return rc;
+    }
     *out = s.release();
     return TFR_OK;
   }
@@ -219,6 +255,8 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
     const tfr_field& f = fields[i];
     if (f.name_len < 0 || (f.name_len > 0 && !f.name)) return fail(TFR_E_INVALID_ARG, "bad field name");
     std::string nm(f.name ? f.name : "", (size_t)f.name_len);
+    int32_t rc = TFR_OK;
+    if (add_generated(*s, f, nm, &rc)) { if (rc) return rc; continue; }
     // newFeatureWriter / newFeatureConverter: anything but these types throws (M/TFRecordDeserializer.scala:119-123,
     // M/TFRecordSerializer.scala:147,151); ArrayType(NullType) falls into the same default branch
     bool ok_type = f.elem_type >= TFR_T_NULL && f.elem_type <= TFR_T_BINARY && f.depth >= 0 && f.depth <= 2 &&
@@ -256,16 +294,17 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
     }
     s->ht[slot] = i;
   }
+  if (s->has_generated()) schema_rehash(*s, -1);         // (after the duplicate-name check, which covers them too)
   *out = s.release();
   return TFR_OK;
 }
-// the key hash table without field `skip`: no feature of the record maps to that field any more, so every kernel writes it as
-// an absent field (a PERMISSIVE decoder's corrupt-record column)
+// the key hash table without field `skip` and the generated fields: no feature of the record maps to them, so every kernel
+// writes them as absent fields (a PERMISSIVE decoder's corrupt-record column; position_kernel then fills the generated ones)
 static void schema_rehash(tfr_schema& s, int32_t skip) {
   std::fill(s.ht.begin(), s.ht.end(), -1);
   const size_t mask = s.ht.size() - 1;
   for (int32_t i = 0; i < (int32_t)s.fields.size(); ++i) {
-    if (i == skip) continue;
+    if (i == skip || s.generated(i)) continue;
     size_t slot = s.fields[i].hash & mask;
     while (s.ht[slot] >= 0) slot = (slot + 1) & mask;
     s.ht[slot] = i;
@@ -302,7 +341,7 @@ struct DevSchemaBuf {
         const DevField& fd = s.fields[f];
         t.kind = (uint32_t)fd.kind;
         const uint32_t klen = fd.name_len, total = klen + 8;
-        if (fd.kind == K_NONE || klen >= 0x80 || total > TILE_TPL_WORDS * 4 || (int32_t)f == unkeyed) continue;      // no template: generic parse
+        if (fd.kind == K_NONE || klen >= 0x80 || total > TILE_TPL_WORDS * 4 || (int32_t)f == unkeyed || s.generated((int32_t)f)) continue;      // no template: generic parse
         uint8_t bytes[TILE_TPL_WORDS * 4] = {0}, mask[TILE_TPL_WORDS * 4] = {0};
         auto put = [&](uint32_t i, uint8_t b, bool fixed) { bytes[i] = b; mask[i] = fixed ? 0xFF : 0x00; };
         put(0, 0x0A, true); put(1, 0, false); put(2, 0x0A, true); put(3, (uint8_t)klen, true);

@@ -29,10 +29,27 @@ import numpy as np
 
 from . import _cabi, _native
 from ._cabi import TFR_F_DEFAULT, TFR_F_DROP_MALFORMED, TFR_F_PERMISSIVE, TFR_F_RESYNC, TFR_E_BATCH_TOO_LARGE as A_TFR_E_BATCH_TOO_LARGE, columns_from_rows
-from .sqltypes import RECORD_TYPES, BinaryType, StructField, StructType, byte_array_schema
+from .sqltypes import (RECORD_TYPES, BinaryType, LongType, RecordOffsetType, RowIndexType, StructField, StructType,
+                       byte_array_schema)
 
 M = "src/main/scala/com/linkedin/spark/datasources/tfrecord/"
 _LOG = logging.getLogger(__name__)
+
+
+# Spark's generated metadata fields (FileFormat.ROW_INDEX, ROW_INDEX_TEMPORARY_COLUMN_NAME in Spark 3.4 / 3.5; restated, not
+# checked against a JVM): `_metadata.row_index` is filled by the reader through a temporary LongType column that Spark adds
+# to the required schema.  record_offset follows the same pattern.  The decoder fills both on the GPU (include/tfrgpu.h,
+# POSITIONS).
+ROW_INDEX, ROW_INDEX_TEMPORARY_COLUMN_NAME = "row_index", "_tmp_metadata_row_index"
+RECORD_OFFSET, RECORD_OFFSET_TEMPORARY_COLUMN_NAME = "record_offset", "_tmp_metadata_record_offset"
+_GENERATED = {ROW_INDEX_TEMPORARY_COLUMN_NAME: RowIndexType(), RECORD_OFFSET_TEMPORARY_COLUMN_NAME: RecordOffsetType()}
+
+
+def _decoder_schema(requiredSchema: StructType) -> StructType:
+    """the required schema as the decoder takes it: Spark's temporary metadata columns (LongType) become generated fields,
+    at their place; every other field is a data field"""
+    return StructType([StructField(f.name, _GENERATED[f.name], False) if f.name in _GENERATED and f.dataType == LongType() else f
+                       for f in requiredSchema])
 
 
 def _record_type(options: Optional[Dict[str, str]]) -> int:
@@ -339,11 +356,14 @@ class TFRecordFileReader:
         row of nulls, its payload in the corrupt-record column when `schema` holds it, and logged the same way.  With
         resyncFraming = "true" as well, a framing error does not raise: the bytes up to the next verified record are a lost
         region, dropped or read as one corrupt row, and each is logged with its file offset and length.
-        `dataSchema` (default: `schema`) is the file's schema, which PERMISSIVE needs the corrupt-record column in."""
+        `dataSchema` (default: `schema`) is the file's schema, which PERMISSIVE needs the corrupt-record column in.
+        A LongType field of `schema` named _tmp_metadata_row_index or _tmp_metadata_record_offset (Spark's temporary
+        metadata columns) holds each row's entry index in the file or the file offset of its entry (in the decompressed
+        stream for a compressed file), filled on the GPU.  ByteArray rows are byteArray, then those fields."""
         rt = _record_type(options)
         flags, corrupt = _read_mode(options, schema if dataSchema is None else dataSchema, schema)
         block = block_bytes or TFRecordFileReader.BLOCK_BYTES
-        dec = _native.Decoder(schema, rt, device, flags, corrupt_field=corrupt)
+        dec = _native.Decoder(_decoder_schema(schema), rt, device, flags, corrupt_field=corrupt)
 
         def gen():
             todo = []
@@ -356,6 +376,7 @@ class TFRecordFileReader:
                     n_slots = dec.num_staging_slots()
                     turn = [0]
                     pos = [0 if compressed else file.start]     # where the next block starts in the (decompressed) file
+                    entries = [0]                               # and the entries in front of it (the file is read whole)
 
                     def stage(nbytes):
                         st = dec.staging_slot(turn[0] % n_slots, nbytes)
@@ -363,10 +384,11 @@ class TFRecordFileReader:
                         return st
 
                     def process(st, nbytes, final):
-                        batch = dec.submit(st, is_final=final, nbytes=nbytes)
+                        batch = dec.submit(st, is_final=final, nbytes=nbytes, first_entry=entries[0], first_offset=pos[0])
                         todo.append((batch, pos[0]))
-                        used = batch.consumed()
+                        used, n = batch.extent()
                         pos[0] += used
+                        entries[0] += n
                         return used
 
                     def drain(batch, block_pos):
@@ -471,6 +493,14 @@ class DefaultSource:
 
     def isSplitable(self, *a, **k) -> bool:
         return False                                             # :26-29; splitting happens inside the native side
+
+    def metadataSchemaFields(self) -> List[Tuple[str, str, "LongType"]]:
+        """The generated metadata fields this source fills, as FileFormat.metadataSchemaFields lists them (Spark 3.4 / 3.5:
+        FileSourceGeneratedMetadataStructField(name, temporary column name, LongType, nullable = false)) on top of Spark's
+        file-constant ones, which Spark appends itself: (name, temporary column, type).  _metadata.row_index is the row's
+        entry index in its file, _metadata.record_offset the file offset of its entry; readFile fills the temporary columns."""
+        return [(ROW_INDEX, ROW_INDEX_TEMPORARY_COLUMN_NAME, LongType()),
+                (RECORD_OFFSET, RECORD_OFFSET_TEMPORARY_COLUMN_NAME, LongType())]
 
     def inferSchema(self, options: Dict[str, str], files: Sequence[str], device: int = 0, dist=None):
         """M/DefaultSource.scala:31-39,48-70: the first non-empty file is scanned (the reference scans it twice);

@@ -13,6 +13,11 @@
 //     static native int stagingSlots();
 //     static native long decode(long decoder, java.nio.ByteBuffer staged, long nbytes, boolean isFinal, long[] consumedOut);
 //     static native long decodeSubmit(long decoder, java.nio.ByteBuffer staged, long nbytes, boolean isFinal);   // pipelined: no wait
+//     static native long decodeAt(long decoder, java.nio.ByteBuffer staged, long nbytes, boolean isFinal, long firstEntry,
+//                                 long firstOffset, long[] consumedOut);   // the block's place in its file: _metadata.row_index
+//     static native long decodeSubmitAt(long decoder, java.nio.ByteBuffer staged, long nbytes, boolean isFinal, long firstEntry,
+//                                       long firstOffset);
+//     static native long[] batchExtent(long batch);   // {consumed, entries}: the next block's firstOffset / firstEntry advance
 //     static native void batchToHostAsync(long batch);                                                            // D2H behind the kernels
 //     static native long[] batchStatus(long batch);      // {nRows, nRecords, consumed, errorCode, errorRow, errorField}; waits for a submitted batch
 //     static native java.nio.ByteBuffer[] batchColumnHost(long batch, int column, long[] meta);  // validity, offsets*, values
@@ -128,6 +133,25 @@ extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_
   if (rc) { throw_for(env, rc, -1); return 0; }
   return (jlong)b;
 }
+// the same two calls for a block at (firstEntry, firstOffset) of its file: the base of the generated metadata columns
+// (_tmp_metadata_row_index, _tmp_metadata_record_offset, lowered to TFR_T_ROW_INDEX / TFR_T_RECORD_OFFSET by schemaCreate)
+extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_decodeAt(
+    JNIEnv* env, jclass, jlong dec, jobject staged, jlong nbytes, jboolean isFinal, jlong firstEntry, jlong firstOffset, jlongArray consumedOut) {
+  void* p = env->GetDirectBufferAddress(staged);
+  tfr_batch* b = nullptr; size_t used = 0;
+  int32_t rc = tfr_decode_at((tfr_decoder*)dec, p, (size_t)nbytes, 0, isFinal ? 1 : 0, (int64_t)firstEntry, (int64_t)firstOffset, &b, &used);
+  if (rc) { throw_for(env, rc, -1); return 0; }
+  jlong u = (jlong)used; env->SetLongArrayRegion(consumedOut, 0, 1, &u);
+  return (jlong)b;
+}
+extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_decodeSubmitAt(
+    JNIEnv* env, jclass, jlong dec, jobject staged, jlong nbytes, jboolean isFinal, jlong firstEntry, jlong firstOffset) {
+  void* p = env->GetDirectBufferAddress(staged);
+  tfr_batch* b = nullptr;
+  int32_t rc = tfr_decode_submit_at((tfr_decoder*)dec, p, (size_t)nbytes, 0, isFinal ? 1 : 0, (int64_t)firstEntry, (int64_t)firstOffset, &b);
+  if (rc) { throw_for(env, rc, -1); return 0; }
+  return (jlong)b;
+}
 extern "C" JNIEXPORT void JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_batchToHostAsync(JNIEnv* env, jclass, jlong batch) {
   int32_t rc = tfr_batch_to_host_async((tfr_batch*)batch);
   if (rc) { tfr_batch_release((tfr_batch*)batch); throw_for(env, rc, -1); }
@@ -138,6 +162,16 @@ extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_
   int32_t rc = tfr_batch_consumed((tfr_batch*)batch, &used);
   if (rc) { tfr_batch_release((tfr_batch*)batch); throw_for(env, rc, -1); return 0; }
   return (jlong)used;
+}
+// batchConsumed plus the entries in the consumed bytes, with the same wait: {consumed, entries}
+extern "C" JNIEXPORT jlongArray JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_batchExtent(JNIEnv* env, jclass, jlong batch) {
+  size_t used = 0; int64_t entries = 0;
+  int32_t rc = tfr_batch_extent((tfr_batch*)batch, &used, &entries);
+  if (rc) { tfr_batch_release((tfr_batch*)batch); throw_for(env, rc, -1); return nullptr; }
+  jlong v[2] = {(jlong)used, (jlong)entries};
+  jlongArray out = env->NewLongArray(2);
+  env->SetLongArrayRegion(out, 0, 2, v);
+  return out;
 }
 extern "C" JNIEXPORT jlongArray JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_batchStatus(JNIEnv* env, jclass, jlong batch) {
   tfr_batch_info i{};

@@ -12,6 +12,7 @@ from typing import List, Sequence
 
 # tfr type ids (include/tfrgpu.h)
 TFR_T_NULL, TFR_T_INT32, TFR_T_INT64, TFR_T_FLOAT32, TFR_T_FLOAT64, TFR_T_DECIMAL, TFR_T_STRING, TFR_T_BINARY = range(8)
+TFR_T_ROW_INDEX, TFR_T_RECORD_OFFSET = 8, 9          # generated fields: read as LongType, never from a record
 TFR_T_UNSUPPORTED = 99
 TFR_RT_EXAMPLE, TFR_RT_SEQUENCE_EXAMPLE, TFR_RT_BYTE_ARRAY = range(3)
 
@@ -63,6 +64,17 @@ class StringType(DataType):
 
 class BinaryType(DataType):
     tfr_id = TFR_T_BINARY
+
+
+class RowIndexType(DataType):
+    """A generated LongType field: the row's entry index in its file (include/tfrgpu.h, POSITIONS).  Not a Spark type: the
+    reader puts it in place of the LongType of Spark's temporary metadata column (io.readFile)."""
+    tfr_id = TFR_T_ROW_INDEX
+
+
+class RecordOffsetType(DataType):
+    """A generated LongType field: the file offset of the row's entry (include/tfrgpu.h, POSITIONS)."""
+    tfr_id = TFR_T_RECORD_OFFSET
 
 
 class TimestampType(DataType):
