@@ -263,7 +263,8 @@ int32_t tfr_decoder_get_profile(tfr_decoder*, double* ms /* [TFR_PROFILE_STAGES]
  * launched with), [9] records dropped (TFR_F_DROP_MALFORMED), [10] records delivered as corrupt rows
  * (TFR_F_PERMISSIVE), [11] lost regions and [12] the bytes in them (TFR_F_RESYNC).  A caller passing n = 8 gets the
  * first eight.  The counters before [11] keep their meaning: n <= 11 gets them all, counter [10] being PERMISSIVE's, and a
- * caller passing 10 or fewer is unaffected; n = 13 adds the two of TFR_F_RESYNC.                                     */
+ * caller passing 10 or fewer is unaffected; n = 13 adds the two of TFR_F_RESYNC.  [13] batches decoded by the
+ * large-record kernel (records too large for a shared-memory tile, csrc/large.cuh); n <= 13 is unaffected by it.       */
 int32_t tfr_decoder_get_stats(tfr_decoder*, int64_t* out, int32_t n /* <= 10 */);
 
 int32_t tfr_batch_wait(tfr_batch*);

@@ -377,11 +377,12 @@ class Decoder:
         return lib().tfr_decoder_num_staging_slots()
 
     def stats(self) -> dict:
-        v = (C.c_int64 * 13)()
-        _check(lib().tfr_decoder_get_stats(self.h, v, 13))
+        v = (C.c_int64 * 14)()
+        _check(lib().tfr_decoder_get_stats(self.h, v, 14))
         names = ["batches", "speculative_submits", "speculative_redone", "count_mode_batches", "general_path_batches", "shapes_learned", "transcode_reruns",
                  "rows_async", "rows_async_rebuilt", "records_dropped", "records_corrupt"]
         names += ["lost_regions", "lost_region_bytes"]                   # TFR_F_RESYNC
+        names += ["large_record_batches"]                               # the large-record kernel (csrc/large.cuh)
         return {k: v[i] for i, k in enumerate(names)}
 
     def stream(self) -> int:

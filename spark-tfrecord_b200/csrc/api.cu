@@ -24,6 +24,7 @@
 #include "frame.cuh"
 #include "host_util.h"
 #include "infer.cuh"
+#include "large.cuh"
 #include "permissive.cuh"
 #include "position.cuh"
 #include "resync.cuh"
@@ -125,6 +126,7 @@ static void build_crc_tables(CrcTables& t) {
     for (int k = 1; k < 8; ++k) t.s8[k][i] = (t.s8[k - 1][i] >> 8) ^ t.t0[t.s8[k - 1][i] & 0xff];
   }
   for (uint32_t m = 0; m < 512; ++m) t.xp16[m] = xpow_bytes(16 * m);
+  for (uint32_t k = 0; k < 32; ++k) t.x8pow[k] = xpow_bytes(1u << k);
   memset(t.g5, 0, sizeof t.g5);
   for (uint32_t k = 0; k < 13; ++k)
     for (uint32_t v = 0; v < 32; ++v) {

@@ -31,6 +31,7 @@ struct CrcTables {
   //   g5[416 + v], g5[448 + w]: the byte-wise table split the same way, t0[x] = g5[416 + (x & 31)] ^ g5[448 + (x >> 5)]
   uint32_t g5[512];
   uint32_t xp16[512];    // x^(8*16*m) mod P: shifts a CRC state over m later 16-byte chunks (contiguous with g5)
+  uint32_t x8pow[32];    // x^(8 * 2^k) mod P: shifts over any number of bytes as a product over its set bits (large.cuh)
 };
 #define CRC_SMEM_WORDS (256 + 1024 + 40)
 
