@@ -69,8 +69,38 @@ enum {
    * refuses a schema that has one (TFR_E_UNSUPPORTED_TYPE).  Their tfr_column reports TFR_T_INT64, depth 0, null_count 0
    * and every validity bit set, so every view of a batch (columns, host copy, Arrow, UnsafeRows) reads them as LongType. */
   TFR_T_ROW_INDEX     = 8,  /* the row's entry index in its file                                */
-  TFR_T_RECORD_OFFSET = 9   /* the file offset of the row's entry                               */
+  TFR_T_RECORD_OFFSET = 9,  /* the file offset of the row's entry                               */
+  TFR_T_VECTOR        = 10  /* Spark ML's VectorUDT, read and written as a FloatList (VECTORS below) */
 };
+/* VECTORS: TFR_T_VECTOR is org.apache.spark.ml.linalg.VectorUDT (and org.apache.spark.mllib.linalg.VectorUDT, which has the
+ * same sqlType: struct<type: tinyint not null, size: int, indices: array<int not null>, values: array<double not null>>).
+ *   - Schema : depth 0 only; at depth 1 or 2 (ArrayType(VectorUDT)) tfr_schema_create returns TFR_E_UNSUPPORTED_TYPE naming
+ *              the field.  Decoders and encoders take it; a ByteArray schema ignores it like any data field; schema inference
+ *              never produces it (a FloatList infers as ArrayType(FloatType)).
+ *   - Read   : the field reads what an ArrayType(DoubleType) field of the same name and nullability reads, by every rule of
+ *              the decoder (kinds, SequenceExample heads, FAILFAST / DROPMALFORMED / PERMISSIVE, TFR_F_RESYNC), as a dense
+ *              vector of those values: null, the error, its row and its field exactly where that field's would be.  Its
+ *              tfr_column is that field's: TFR_T_FLOAT64, depth 1, n_levels 1 (host copy and Arrow export: list<double>).
+ *   - Rows   : tfr_batch_rows (and _with_partition, _async) write what UnsafeProjection makes of
+ *              VectorUDT.serialize(DenseVector(values)): the slot is (offset << 32) | size of a nested UnsafeRow of 4 fields:
+ *              one null word with bits 1 and 2 set, the slots type = 1 (the low byte; the other bytes zero), size = 0,
+ *              indices = 0, values = (40 << 32) | bytes (offset from the nested row), then the values' UnsafeArrayData
+ *              (numElements, a zero element null bitset, the doubles).  A null vector has its bit set and a zero slot.
+ *   - Write, tfr_encode : the column is list<double> of the dense values (TFR_T_FLOAT64, depth 1); the output is byte-identical
+ *              to the same column as ArrayType(DoubleType).
+ *   - Write, tfr_encode_rows / tfr_encode_rows_submit : the struct above, encoded as ArrayType(DoubleType) encodes
+ *              vector.toArray (each element through toFloat): type 1 (dense) gives `values`; type 0 (sparse) gives `size` zeros
+ *              (+0.0f) with values(i) at indices(i).  A null vector is omitted, or TFR_E_NULL_IN_NONNULL in a non-nullable
+ *              field.  TFR_E_INVALID_ARG (a malformed row, with the existing precedence over a null): a struct slot outside
+ *              its row, misaligned or shorter than the 40-byte fixed part; a type other than 0 or 1 (MatchError in
+ *              VectorUDT.deserialize); a null `values`, or a null `indices` when sparse (NullPointerException); a malformed
+ *              inner array; a sparse vector with size < 0, indices and values of different lengths, or an index outside
+ *              [0, size) or not strictly increasing (the requires of SparseVector's constructor).  The type and size slots
+ *              are read whatever their null bits (getByte / getInt); the element null bits of indices and values are ignored
+ *              and their slots' bits copied (toIntArray / toDoubleArray).  A batch whose densified values exceed the
+ *              encoder's limits is TFR_E_BATCH_TOO_LARGE with no output.
+ * These rules are restated from Spark's sources (VectorUDT.serialize / deserialize, SparseVector's constructor,
+ * UnsafeRowWriter for a nested struct) and are NOT checked against a JVM, like the partition-row and float-bits rules.  */
 
 /* record types: the `recordType` DataSource option (M/TFRecordFileReader.scala:22,69-80) */
 enum { TFR_RT_EXAMPLE = 0, TFR_RT_SEQUENCE_EXAMPLE = 1, TFR_RT_BYTE_ARRAY = 2 };
@@ -81,7 +111,7 @@ typedef struct tfr_field {
   const char* name;      /* UTF-8 bytes, not necessarily NUL terminated */
   int32_t     name_len;
   int32_t     elem_type; /* TFR_T_*  */
-  int32_t     depth;     /* 0, 1, 2  */
+  int32_t     depth;     /* 0, 1, 2 (TFR_T_VECTOR: 0) */
   int32_t     nullable;  /* StructField.nullable */
 } tfr_field;
 

@@ -9,7 +9,8 @@ from typing import List, Sequence
 import numpy as np
 
 from .sqltypes import (StructType, lower_type, TFR_T_NULL, TFR_T_INT32, TFR_T_INT64, TFR_T_FLOAT32,
-                       TFR_T_FLOAT64, TFR_T_DECIMAL, TFR_T_STRING, TFR_T_BINARY, TFR_T_ROW_INDEX, TFR_T_RECORD_OFFSET)
+                       TFR_T_FLOAT64, TFR_T_DECIMAL, TFR_T_STRING, TFR_T_BINARY, TFR_T_ROW_INDEX, TFR_T_RECORD_OFFSET,
+                       TFR_T_VECTOR)
 
 TFR_OK = 0
 TFR_E_INVALID_ARG = -1
@@ -169,11 +170,15 @@ def column_from_ctypes(c: tfr_column) -> HostColumn:
 def columns_from_rows(schema: StructType, rows: Sequence[Sequence], record_type: int = 0) -> List[HostColumn]:
     """Row-major Python values -> columnar HostColumns (what TFRecordOutputWriter buffers before
     handing a batch to tfr_encode).  Values follow Spark's external types: int, float, str,
-    bytes, list, list of lists; None = null."""
+    bytes, list, list of lists, a DenseVector or SparseVector for VectorUDT (its toArray, as a list<double> column);
+    None = null."""
     cols = []
     n = len(rows)
     for ci, f in enumerate(schema):
         t, depth = lower_type(f.dataType)
+        vector = t == TFR_T_VECTOR and depth == 0
+        if vector:
+            t, depth = TFR_T_FLOAT64, 1
         dt = _LEAF_DTYPE.get(t, np.uint8)
         varlen = t in (TFR_T_STRING, TFR_T_BINARY)
         nlev = depth + (1 if varlen else 0)
@@ -207,7 +212,7 @@ def columns_from_rows(schema: StructType, rows: Sequence[Sequence], record_type:
             if depth == 0:
                 put_leaf(v)
             elif depth == 1:
-                for e in v:
+                for e in (v.toArray().tolist() if vector else v):
                     put_leaf(e)
                 offs[0].append(leaf_count())
             else:

@@ -196,6 +196,11 @@ struct tfr_schema {
   int32_t gen_field[2] = {-1, -1};
   bool generated(int32_t f) const { return f >= 0 && (f == gen_field[0] || f == gen_field[1]); }
   bool has_generated() const { return gen_field[0] >= 0 || gen_field[1] >= 0; }
+  // TFR_T_VECTOR fields (include/tfrgpu.h, VECTORS): 1 per such field, else 0.  Lowered to float64 depth-1 fields, so every
+  // parse and encode kernel treats them as ArrayType(DoubleType); only the UnsafeRow kernels (urows.cuh, rows.cuh) read this.
+  std::vector<uint8_t> vec;
+  bool vector(int32_t f) const { return f >= 0 && f < (int32_t)vec.size() && vec[f]; }
+  bool has_vector() const { return std::find(vec.begin(), vec.end(), 1) != vec.end(); }
 };
 
 static uint32_t fnv1a(const uint8_t* p, uint32_t n) { uint32_t h = 2166136261u; for (uint32_t i = 0; i < n; ++i) h = (h ^ p[i]) * 16777619u; return h; }
@@ -250,6 +255,7 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
       add_generated(*s, f, std::string(f.name ? f.name : "", (size_t)f.name_len), &rc);
       if (rc) return rc;
     }
+    s->vec.assign(s->fields.size(), 0);
     *out = s.release();
     return TFR_OK;
   }
@@ -258,29 +264,35 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
     if (f.name_len < 0 || (f.name_len > 0 && !f.name)) return fail(TFR_E_INVALID_ARG, "bad field name");
     std::string nm(f.name ? f.name : "", (size_t)f.name_len);
     int32_t rc = TFR_OK;
+    s->vec.resize(s->fields.size(), 0);
     if (add_generated(*s, f, nm, &rc)) { if (rc) return rc; continue; }
+    // a VectorUDT field is an ArrayType(DoubleType) field to every kernel but the UnsafeRow ones (VECTORS)
+    const bool vector = f.elem_type == TFR_T_VECTOR;
+    if (vector && f.depth != 0) return fail(TFR_E_UNSUPPORTED_TYPE, "field '" + nm + "': ArrayType(VectorUDT) is not supported");
+    const int32_t et = vector ? TFR_T_FLOAT64 : f.elem_type, depth = vector ? 1 : f.depth;
     // newFeatureWriter / newFeatureConverter: anything but these types throws (M/TFRecordDeserializer.scala:119-123,
     // M/TFRecordSerializer.scala:147,151); ArrayType(NullType) falls into the same default branch
-    bool ok_type = f.elem_type >= TFR_T_NULL && f.elem_type <= TFR_T_BINARY && f.depth >= 0 && f.depth <= 2 &&
-                   !(f.elem_type == TFR_T_NULL && f.depth > 0);
+    bool ok_type = et >= TFR_T_NULL && et <= TFR_T_BINARY && depth >= 0 && depth <= 2 && !(et == TFR_T_NULL && depth > 0);
     if (!ok_type) return fail(TFR_E_UNSUPPORTED_TYPE, "field '" + nm + "': data type is not supported");
     DevField d{};
     d.name_off = (uint32_t)s->names.size();
     d.name_len = (uint32_t)f.name_len;
     s->names.insert(s->names.end(), (const uint8_t*)f.name, (const uint8_t*)f.name + f.name_len);
     d.hash = fnv1a((const uint8_t*)f.name, d.name_len);
-    d.elem_type = (int8_t)f.elem_type; d.depth = (int8_t)f.depth; d.nullable = f.nullable ? 1 : 0;
-    d.kind = (int8_t)required_kind(f.elem_type);
-    bool varlen = f.elem_type == TFR_T_STRING || f.elem_type == TFR_T_BINARY;
-    d.n_levels = (int16_t)(f.depth + (varlen ? 1 : 0));
+    d.elem_type = (int8_t)et; d.depth = (int8_t)depth; d.nullable = f.nullable ? 1 : 0;
+    d.kind = (int8_t)required_kind(et);
+    bool varlen = et == TFR_T_STRING || et == TFR_T_BINARY;
+    d.n_levels = (int16_t)(depth + (varlen ? 1 : 0));
     d.dup_next = -1;
-    d.width = type_width(f.elem_type);
+    d.width = type_width(et);
     d.fix_slot = -1; d.var_slot = -1; d.cnt_slot = -1;
+    s->vec.push_back(vector ? 1 : 0);
     if (f.elem_type == TFR_T_NULL) { /* no storage beyond validity */ }
     else if (d.n_levels == 0) { d.fix_slot = s->n_fix++; s->fix_field.push_back(i); }
     else { d.var_slot = s->n_var++; d.cnt_slot = s->n_cnt; s->n_cnt += d.n_levels; s->var_field.push_back(i); }
     s->fields.push_back(d);
   }
+  s->vec.resize(s->fields.size(), 0);
   // Spark refuses duplicate column names for file sources before the reader is built
   // (SchemaUtils.checkColumnNameDuplication), so they never reach TFRecordDeserializer
   size_t hsz = 2; while (hsz < 2 * (size_t)n_fields + 2) hsz <<= 1;
@@ -319,9 +331,11 @@ extern "C" int32_t tfr_schema_num_fields(const tfr_schema* s) { return s ? (int3
 // kernels run on non-blocking streams, which nothing orders after the legacy default stream, and `tp` is a local.
 struct DevSchemaBuf {
   DevBuf fields, names, ht, var_field, templates;
+  DevBuf vec;                                             // tfr_schema::vec, for the UnsafeRow kernels of the encoder
   DevBuf tile_consts; uint32_t tile_consts_bytes = 0;     // tile.cuh: per-schema constants in the shared-memory layout
   DevSchema view{};
   const int32_t* d_var_field() const { return (const int32_t*)var_field.p; }
+  const uint8_t* d_vec() const { return (const uint8_t*)vec.p; }
   const uint8_t* d_tile_consts() const { return (const uint8_t*)tile_consts.p; }
   // `unkeyed`: a field no feature maps to (schema_rehash), which gets no entry template either
   int32_t upload(const tfr_schema& s, cudaStream_t st, int32_t unkeyed = -1) {
@@ -330,7 +344,9 @@ struct DevSchemaBuf {
     CUDA_TRY(names.alloc(std::max<size_t>(1, s.names.size())));
     CUDA_TRY(ht.alloc(s.ht.size() * sizeof(int32_t)));
     CUDA_TRY(var_field.alloc(std::max<size_t>(1, s.var_field.size()) * sizeof(int32_t)));
+    CUDA_TRY(vec.alloc(std::max<size_t>(1, nf)));
     if (nf) CUDA_TRY(cudaMemcpyAsync(fields.p, s.fields.data(), nf * sizeof(DevField), cudaMemcpyHostToDevice, st));
+    if (!s.vec.empty()) CUDA_TRY(cudaMemcpyAsync(vec.p, s.vec.data(), s.vec.size(), cudaMemcpyHostToDevice, st));
     if (!s.names.empty()) CUDA_TRY(cudaMemcpyAsync(names.p, s.names.data(), s.names.size(), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(ht.p, s.ht.data(), s.ht.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     if (!s.var_field.empty()) CUDA_TRY(cudaMemcpyAsync(var_field.p, s.var_field.data(), s.var_field.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));

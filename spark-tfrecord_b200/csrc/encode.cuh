@@ -33,12 +33,14 @@ struct EncStatus {
   uint32_t rows_first_bad;      // row kernels, atomicMin: first malformed row
   uint32_t rows_first_null;     // row kernels, atomicMin: first row with a null element
   uint32_t rows_overflow;       // row kernels: a scan of counts overflowed or an arena is too small
-  uint32_t pad1[5];
+  uint32_t rows_vec_lo, rows_vec_hi;   // rows_layout_kernel: the dense values of the batch's vector fields
+  uint32_t pad1[3];
   uint32_t verdict_flag;        // encode_verdict_kernel: EVF_* (0: the batch can be emitted as launched)
   uint32_t verdict_total_lo, verdict_total_hi;   // and the batch's framed bytes
   uint32_t pad2[13];
   uint64_t total() const { return total_lo | (uint64_t)total_hi << 32; }
   uint64_t verdict_total() const { return verdict_total_lo | (uint64_t)verdict_total_hi << 32; }
+  uint64_t rows_vec() const { return rows_vec_lo | (uint64_t)rows_vec_hi << 32; }
 };
 static_assert(sizeof(EncStatus) == 128, "the status block is copied whole");
 static_assert(offsetof(EncStatus, total_lo) % 8 == 0, "the host copies a 64-bit scan total onto total_lo / total_hi");

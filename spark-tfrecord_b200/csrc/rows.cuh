@@ -39,7 +39,8 @@ struct RowsArgs {
   int32_t* const* lev;          // [n_cnt] scan outputs: level 0 = the column's Arrow offsets, levels 1, 2 = per-row bases
   EncCol* cols;                 // [n_fields] the encoder's columns; the layout kernel fills the inner offsets and values
   uint32_t smem_cap;            // tile bytes the shared-memory staging holds
-  EncStatus* st;                // rows_first_bad, rows_first_null, rows_overflow
+  EncStatus* st;                // rows_first_bad, rows_first_null, rows_overflow, rows_vec_lo / hi
+  const uint8_t* vec;           // [n_fields] 1: a VectorUDT field (a float64 list column filled from the struct)
 };
 
 enum { RW_OK = 0, RW_NULL = 1, RW_BAD = 2 };
@@ -129,6 +130,52 @@ __device__ int rows_field_counts(const uint8_t* row, uint64_t len, const DevFiel
   return st;
 }
 
+// A VectorUDT value (include/tfrgpu.h, VECTORS): the nested UnsafeRow struct<type: tinyint, size: int, indices: array<int>,
+// values: array<double>> of `slot`.  Its dense length (`size` when sparse) and where its arrays' elements start, row-relative.
+struct RowsVec {
+  bool sparse;
+  uint32_t n, size;             // values (and indices) elements; the dense length
+  uint64_t vals, idx;
+};
+// RW_OK or RW_BAD (VectorUDT.deserialize and SparseVector's constructor would throw).  `check`: the indices are checked too
+// (pass A); pass B reads only rows pass A found well-formed.
+__device__ int rows_vector(const uint8_t* row, uint64_t len, uint64_t slot, bool check, RowsVec& v) {
+  const uint64_t o = slot >> 32, sz = slot & 0xffffffffu;
+  if ((o & 7) || o + sz > len || sz < 40) return RW_BAD;
+  const uint64_t nulls = rows_ld64(row + o);
+  const int8_t type = (int8_t)row[o + 8];                   // getByte(0), whatever its null bit
+  if (type != 0 && type != 1) return RW_BAD;                // MatchError
+  v.sparse = type == 0;
+  uint64_t eo, es;
+  if ((nulls >> 3) & 1 || !rows_var_elem(row, o, sz, o + 8, 3, eo, es) || !rows_array(row, eo, es, 8, v.n, v.vals)) return RW_BAD;
+  if (!v.sparse) { v.size = v.n; return RW_OK; }
+  const int32_t size = (int32_t)(uint32_t)rows_ld64(row + o + 16);      // getInt(1)
+  uint32_t m;
+  if (size < 0 || (nulls >> 2) & 1 || !rows_var_elem(row, o, sz, o + 8, 2, eo, es) || !rows_array(row, eo, es, 4, m, v.idx) || m != v.n)
+    return RW_BAD;
+  v.size = (uint32_t)size;
+  if (check) {
+    int64_t prev = -1;
+    for (uint32_t i = 0; i < m; ++i) {
+      const int32_t k = reinterpret_cast<const int32_t*>(row + v.idx)[i];
+      if (k <= prev || k >= size) return RW_BAD;            // strictly increasing, inside [0, size)
+      prev = k;
+    }
+  }
+  return RW_OK;
+}
+
+// The counts of a field: a vector's level 0 is its dense length.  Its values go to an arena of their own, sized from the
+// scanned counts, so they add nothing to `room`.
+__device__ __forceinline__ int rows_counts(const RowsArgs& A, uint32_t f, const uint8_t* row, uint64_t len, const DevField& fd, uint64_t slot,
+                                           uint32_t c[3], uint64_t& room) {
+  if (!A.vec[f]) return rows_field_counts(row, len, fd, slot, c, room);
+  RowsVec v;
+  if (rows_vector(row, len, slot, true, v) != RW_OK) return RW_BAD;
+  c[0] = v.size;
+  return RW_OK;
+}
+
 __device__ __forceinline__ bool rows_field_null(const uint8_t* row, uint32_t f) { return (rows_ld64(row + 8ull * (f >> 6)) >> (f & 63)) & 1; }
 
 __global__ void __launch_bounds__(ROWS_TILE) rows_pass_a_kernel(RowsArgs A) {
@@ -175,7 +222,7 @@ __global__ void __launch_bounds__(ROWS_TILE) rows_pass_a_kernel(RowsArgs A) {
       const DevField& fd = A.sch.fields[f];
       if (fd.n_levels == 0 || rows_field_null(row, f)) continue;
       uint32_t c[3];
-      const int st = rows_field_counts(row, len, fd, rows_ld64(row + 8ull * (nw + f)), c, room);
+      const int st = rows_counts(A, f, row, len, fd, rows_ld64(row + 8ull * (nw + f)), c, room);
       if (st == RW_BAD) { bad = true; break; }
       if (st == RW_NULL) nul = true;
     }
@@ -204,7 +251,7 @@ __global__ void __launch_bounds__(ROWS_TILE) rows_pass_a_kernel(RowsArgs A) {
     }
     uint32_t c[3] = {0, 0, 0};
     uint64_t room = 0;
-    if (present) rows_field_counts(row, len, fd, rows_ld64(row + 8ull * (nw + f)), c, room);
+    if (present) rows_counts(A, f, row, len, fd, rows_ld64(row + 8ull * (nw + f)), c, room);
     for (int l = 0; l < fd.n_levels; ++l) A.cnt[(size_t)(fd.cnt_slot + l) * A.n_rows + r] = c[l];
   }
 }
@@ -216,24 +263,39 @@ __global__ void __launch_bounds__(ROWS_TILE) rows_pass_a_kernel(RowsArgs A) {
 // raised and every variable column becomes all-null AND empty -- validity and level-0 offsets all zero -- so that no
 // kernel, including the ByteArray one that reads only the offsets, touches the unplaced buffers; the host reports the
 // malformed row.  Every block recomputes the totals; block 0 writes.
+// Vector fields (dense lengths, which the input does not bound) go to their own arena `xarena` (xcap bytes), sized by the host
+// from the scanned counts (rows_vec_bytes).  Block 0 stores their values' total in rows_vec_lo / hi.  A pipelined batch sizes
+// that arena from what the encoder learned: a batch it is too small for raises the overflow flag, which the encode's verdict
+// turns into a redo (EVF_ROWS), and the synchronous path then sizes it from the counts.
+__host__ __device__ __forceinline__ unsigned long long rows_vec_place(unsigned long long xpos, unsigned long long values) {
+  return ((xpos + 15) & ~15ull) + values * 8ull;
+}
 __global__ void rows_layout_kernel(RowsArgs A, const unsigned long long* __restrict__ totals, uint8_t* varena, unsigned long long vcap,
-                                   int32_t* iarena, unsigned long long icap) {
+                                   int32_t* iarena, unsigned long long icap, uint8_t* xarena, unsigned long long xcap) {
   __shared__ uint32_t over;
   const uint32_t nf = (uint32_t)A.sch.n_fields;
   if (threadIdx.x == 0) {
-    unsigned long long vpos = 0, ipos = 0;
+    unsigned long long vpos = 0, ipos = 0, xpos = 0, xn = 0;
     for (uint32_t f = 0; f < nf; ++f) {
       const DevField& fd = A.sch.fields[f];
       if (fd.n_levels == 0) continue;
+      if (A.vec[f]) { xpos = rows_vec_place(xpos, totals[fd.cnt_slot]); xn += totals[fd.cnt_slot]; continue; }
       for (int l = 1; l < fd.n_levels; ++l) ipos += totals[fd.cnt_slot + l - 1] + 1;
       vpos = ((vpos + 15) & ~15ull) + totals[fd.cnt_slot + fd.n_levels - 1] * (unsigned long long)fd.width;
     }
-    over = (A.st->rows_overflow != 0 || vpos > vcap || ipos > icap) ? 1u : 0u;
+    over = (A.st->rows_overflow != 0 || vpos > vcap || ipos > icap || xpos > xcap) ? 1u : 0u;
+    if (blockIdx.x == 0) { A.st->rows_vec_lo = (uint32_t)xn; A.st->rows_vec_hi = (uint32_t)(xn >> 32); }
     if (!over && blockIdx.x == 0) {
-      vpos = ipos = 0;
+      vpos = ipos = xpos = 0;
       for (uint32_t f = 0; f < nf; ++f) {
         const DevField& fd = A.sch.fields[f];
         if (fd.n_levels == 0) continue;
+        if (A.vec[f]) {
+          xpos = (xpos + 15) & ~15ull;
+          A.cols[f].values = xarena + xpos;
+          xpos = rows_vec_place(xpos, totals[fd.cnt_slot]);
+          continue;
+        }
         for (int l = 1; l < fd.n_levels; ++l) {
           int32_t* o = iarena + ipos;
           const unsigned long long parents = totals[fd.cnt_slot + l - 1];
@@ -300,6 +362,37 @@ __device__ __forceinline__ void rows_copy_elems(const DevField& fd, void* values
   }
 }
 
+// A vector's dense values (toArray) from index 0 of `out`; warp-uniform call, `act`: this lane has a (well-formed) vector.
+// Dense: its lane copies the values, like a double array.  Sparse: a zero-fill of the dense range, then the scatter of the
+// non-zeros; a range of ROWS_VEC_WARP values or more is filled and scattered by the whole warp (HashingTF's are 2^18 long).
+#define ROWS_VEC_WARP 64u
+__device__ __forceinline__ void rows_vector_fill(const uint8_t* row, uint64_t slot, unsigned long long* out, bool act) {
+  const uint32_t lane = threadIdx.x & 31;
+  RowsVec v{};
+  if (act) rows_vector(row, ~0ull, slot, false, v);
+  const bool big = act && v.sparse && v.size >= ROWS_VEC_WARP;
+  if (act && !big) {
+    if (v.sparse) for (uint32_t i = 0; i < v.size; ++i) out[i] = 0;
+    for (uint32_t i = 0; i < v.n; ++i) {
+      const uint32_t k = v.sparse ? (uint32_t)reinterpret_cast<const int32_t*>(row + v.idx)[i] : i;
+      out[k] = rows_ld64(row + v.vals + 8ull * i);        // a null element keeps its slot's bits (toDoubleArray)
+    }
+  }
+  uint32_t m = __ballot_sync(FULLMASK, big);
+  while (m) {
+    const int l = __ffs(m) - 1;
+    m &= m - 1;
+    unsigned long long* o = (unsigned long long*)__shfl_sync(FULLMASK, (unsigned long long)out, l);
+    const uint8_t* rw = (const uint8_t*)__shfl_sync(FULLMASK, (unsigned long long)row, l);
+    const uint32_t size = __shfl_sync(FULLMASK, v.size, l), n = __shfl_sync(FULLMASK, v.n, l);
+    const uint64_t vals = __shfl_sync(FULLMASK, v.vals, l), idx = __shfl_sync(FULLMASK, v.idx, l);
+    for (uint32_t k = lane; k < size; k += 32) o[k] = 0;
+    __syncwarp();                                           // (orders the zeros before the scatter)
+    for (uint32_t i = lane; i < n; i += 32) o[reinterpret_cast<const int32_t*>(rw + idx)[i]] = rows_ld64(rw + vals + 8ull * i);
+    __syncwarp();
+  }
+}
+
 __global__ void __launch_bounds__(ROWS_B_WARPS * 32) rows_pass_b_kernel(RowsArgs A) {
   if (A.st->rows_overflow) return;                                   // the columns were not placed: nothing to fill
   const uint32_t lane = threadIdx.x & 31;
@@ -319,6 +412,7 @@ __global__ void __launch_bounds__(ROWS_B_WARPS * 32) rows_pass_b_kernel(RowsArgs
     const uint64_t slot = v ? rows_ld64(row + 8ull * (nw + f)) : 0;
     const uint64_t o = slot >> 32, sz = slot & 0xffffffffu;
     const int32_t e0 = v ? A.lev[fd.cnt_slot][r] : 0;
+    if (A.vec[f]) { rows_vector_fill(row, slot, reinterpret_cast<unsigned long long*>(values) + e0, v); continue; }
     if (fd.depth == 0) { rows_copy(values + e0, row + o, (uint32_t)sz, v); continue; }
     if (!v) continue;
     const bool var = rows_is_var(fd);

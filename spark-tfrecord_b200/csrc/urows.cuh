@@ -39,7 +39,9 @@
 #define UROWS_SIZE_THREADS 256
 #define UROWS_BIG 256u
 
-enum { UR_NULL = 0, UR_FIX4 = 1, UR_FIX8 = 2, UR_BYTES = 3, UR_ARR = 4, UR_ARR2 = 5 };
+// UR_VEC: a VectorUDT field (include/tfrgpu.h, VECTORS), a float64 list column written as the nested row of a dense vector
+enum { UR_NULL = 0, UR_FIX4 = 1, UR_FIX8 = 2, UR_BYTES = 3, UR_ARR = 4, UR_ARR2 = 5, UR_VEC = 6 };
+#define UR_VEC_HEAD 40u         // the nested row's fixed part: one null word and four slots
 
 struct UrCol {                  // one decoded column (tfr_column), device pointers
   const uint32_t* valid;        // Arrow validity as 32-bit words
@@ -92,6 +94,7 @@ __device__ __forceinline__ uint64_t ur_value_bytes(const UrCol& c, uint32_t r) {
   const int64_t a = o0[r], b = o0[r + 1];
   if (c.kind == UR_BYTES) return (uint64_t)(b - a);
   if (c.kind == UR_ARR) return ur_arr1_bytes(c, 0, a, b);
+  if (c.kind == UR_VEC) return UR_VEC_HEAD + ur_arr1_bytes(c, 0, a, b);
   uint64_t s = ur_hdr((uint64_t)(b - a)) + 8 * (uint64_t)(b - a);          // UR_ARR2: steps are inner arrays
   const int32_t* o1 = c.off[1];
   for (int64_t k = a; k < b; ++k) s += ur_arr1_bytes(c, 1, o1[k], o1[k + 1]);
@@ -147,6 +150,14 @@ __device__ __forceinline__ void ur_copy_elems(uint8_t* dst, const uint8_t* src, 
 }
 __device__ __forceinline__ void ur_st64(uint8_t* p, uint64_t v) { *reinterpret_cast<unsigned long long*>(p) = v; }
 
+// the fixed part of a dense vector's nested row at dst (zeroed) whose values array has `arr` bytes: null bits 1 (size) and 2
+// (indices), type = 1, size and indices zero slots, values = (40 << 32) | arr
+__device__ __forceinline__ void ur_vec_head(uint8_t* dst, uint64_t arr) {
+  ur_st64(dst, 0x6ull);
+  ur_st64(dst + 8, 1ull);
+  ur_st64(dst + 32, ((uint64_t)UR_VEC_HEAD << 32) | arr);
+}
+
 // one lane writes the 1-D array of elements [e0, e1) of level lvl + 1 at dst (zeroed); returns its bytes
 __device__ uint64_t ur_emit_arr1_lane(const UrCol& c, int lvl, int64_t e0, int64_t e1, uint8_t* dst) {
   const uint64_t m = (uint64_t)(e1 - e0), h = ur_hdr(m);
@@ -180,8 +191,12 @@ __device__ void ur_emit_warp(const UrCol& c, uint32_t r, uint8_t* dst) {
   const int64_t a = c.off[0][r], b = c.off[0][r + 1];
   if (c.kind == UR_BYTES) { ur_copy_bytes(dst, c.values + a, (uint64_t)(b - a), lane, 32); return; }
   const uint64_t m = (uint64_t)(b - a), h = ur_hdr(m);
+  if (c.kind == UR_VEC) {                                  // the nested row's fixed part, then its values array as UR_ARR's
+    if (lane == 0) ur_vec_head(dst, ur_arr1_bytes(c, 0, a, b));
+    dst += UR_VEC_HEAD;
+  }
   if (lane == 0) ur_st64(dst, m);
-  if (c.kind == UR_ARR && c.width) { ur_copy_elems(dst + h, c.values + (uint64_t)a * c.width, m, c.width, lane, 32); return; }
+  if ((c.kind == UR_ARR || c.kind == UR_VEC) && c.width) { ur_copy_elems(dst + h, c.values + (uint64_t)a * c.width, m, c.width, lane, 32); return; }
   // elements with an (offset << 32 | size) slot each: strings / binaries (UR_ARR) or inner arrays (UR_ARR2).  32 at a time,
   // each lane sizes its element, a scan places them, each lane writes its element
   uint64_t base = h + 8 * m;
@@ -205,6 +220,7 @@ __device__ void ur_emit_lane(const UrCol& c, uint32_t r, uint8_t* dst) {
   const int64_t a = c.off[0][r], b = c.off[0][r + 1];
   if (c.kind == UR_BYTES) { ur_copy_bytes(dst, c.values + a, (uint64_t)(b - a), 0, 1); return; }
   if (c.kind == UR_ARR) { ur_emit_arr1_lane(c, 0, a, b, dst); return; }
+  if (c.kind == UR_VEC) { ur_vec_head(dst, ur_emit_arr1_lane(c, 0, a, b, dst + UR_VEC_HEAD)); return; }
   const uint64_t m = (uint64_t)(b - a), h = ur_hdr(m);
   ur_st64(dst, m);
   uint64_t p = h + 8 * m;

@@ -29,8 +29,8 @@ import numpy as np
 
 from . import _cabi, _native
 from ._cabi import TFR_F_DEFAULT, TFR_F_DROP_MALFORMED, TFR_F_PERMISSIVE, TFR_F_RESYNC, TFR_E_BATCH_TOO_LARGE as A_TFR_E_BATCH_TOO_LARGE, columns_from_rows
-from .sqltypes import (RECORD_TYPES, BinaryType, LongType, RecordOffsetType, RowIndexType, StructField, StructType,
-                       byte_array_schema)
+from .sqltypes import (RECORD_TYPES, BinaryType, DenseVector, LongType, RecordOffsetType, RowIndexType, SparseVector, StructField,
+                       StructType, VectorUDT, byte_array_schema)
 
 M = "src/main/scala/com/linkedin/spark/datasources/tfrecord/"
 _LOG = logging.getLogger(__name__)
@@ -229,9 +229,12 @@ def _open_write(path: str, codec: Optional[str]):
     return open(path, "wb")
 
 
-def _rows_of(batch: "_native.Batch") -> List[tuple]:
+def _rows_of(batch: "_native.Batch", schema: Optional[StructType] = None) -> List[tuple]:
+    """the batch's rows; a VectorUDT field of `schema` (the decoder's, Example or SequenceExample) becomes a DenseVector"""
     cols = batch.to_host()
-    return [tuple(c.get(r) for c in cols) for r in range(batch.n_rows)]
+    vec = [isinstance(f.dataType, VectorUDT) for f in schema] if schema is not None else [False] * len(cols)
+    return [tuple(DenseVector(v) if (vec[i] and v is not None) else v for i, v in enumerate(c.get(r) for c in cols))
+            for r in range(batch.n_rows)]
 
 
 class TFRecordDeserializer:
@@ -253,7 +256,7 @@ class TFRecordDeserializer:
         batch, _ = self._decoder(rt).decode(frame)
         try:
             batch.raise_if_error()
-            return _rows_of(batch)[0]
+            return _rows_of(batch, self.schema if rt != 2 else None)[0]
         finally:
             batch.release()
 
@@ -393,7 +396,7 @@ class TFRecordFileReader:
 
                     def drain(batch, block_pos):
                         try:
-                            for row in _rows_of(batch):
+                            for row in _rows_of(batch, schema if rt != 2 else None):
                                 yield row
                             if flags & (TFR_F_DROP_MALFORMED | TFR_F_PERMISSIVE):
                                 dropped = batch.dropped()
@@ -435,6 +438,8 @@ def _row_bytes(row) -> int:
             continue
         if isinstance(v, (bytes, bytearray, str)):
             n += len(v) + 8
+        elif isinstance(v, (DenseVector, SparseVector)):
+            n += 8 * v.size + 8                                  # written dense (toArray)
         elif isinstance(v, (list, tuple)):
             n += 8 + sum((len(x) + 8) if isinstance(x, (bytes, bytearray, str)) else (8 * len(x) + 8 if isinstance(x, (list, tuple)) else 8) for x in v)
         else:

@@ -5,6 +5,7 @@
 // Java side (package com.linkedin.spark.datasources.tfrecord):
 //   final class TfrGpu {
 //     static native long schemaCreate(String[] names, int[] elemTypes, int[] depths, boolean[] nullable, int recordType);
+//     static native int udtElemType(String udtClassName);   // a UserDefinedType's TFR_T_* by class name (VectorUDT: 10), -1 none
 //     static native void schemaDestroy(long schema);
 //     static native long decoderCreate(long schema, int device, int flags);
 //     static native long decoderCreatePermissive(long schema, int device, int flags, int corruptField);   // mode=PERMISSIVE; -1: no corrupt column
@@ -88,6 +89,14 @@ extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_
   env->ReleaseBooleanArrayElements(nullable, nl, JNI_ABORT);
   if (rc) { throw_for(env, rc, -1); return 0; }
   return (jlong)out;
+}
+// The element type of a UserDefinedType field, by the UDT's class name, so that the glue needs no compile-time dependency on
+// spark-mllib: both VectorUDTs (same sqlType) are TFR_T_VECTOR; any other UDT is -1 (unsupported, as in the reference).
+extern "C" JNIEXPORT jint JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_udtElemType(JNIEnv* env, jclass, jstring className) {
+  const char* u = env->GetStringUTFChars(className, nullptr);
+  const std::string name = u ? u : "";
+  if (u) env->ReleaseStringUTFChars(className, u);
+  return name == "org.apache.spark.ml.linalg.VectorUDT" || name == "org.apache.spark.mllib.linalg.VectorUDT" ? TFR_T_VECTOR : -1;
 }
 extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_decoderCreate(JNIEnv* env, jclass, jlong schema, jint device, jint flags) {
   tfr_decoder* d = nullptr;

@@ -10,9 +10,12 @@ from __future__ import annotations
 from dataclasses import dataclass
 from typing import List, Sequence
 
+import numpy as np
+
 # tfr type ids (include/tfrgpu.h)
 TFR_T_NULL, TFR_T_INT32, TFR_T_INT64, TFR_T_FLOAT32, TFR_T_FLOAT64, TFR_T_DECIMAL, TFR_T_STRING, TFR_T_BINARY = range(8)
 TFR_T_ROW_INDEX, TFR_T_RECORD_OFFSET = 8, 9          # generated fields: read as LongType, never from a record
+TFR_T_VECTOR = 10                                      # Spark ML's VectorUDT (include/tfrgpu.h, VECTORS)
 TFR_T_UNSUPPORTED = 99
 TFR_RT_EXAMPLE, TFR_RT_SEQUENCE_EXAMPLE, TFR_RT_BYTE_ARRAY = range(3)
 
@@ -77,6 +80,71 @@ class RecordOffsetType(DataType):
     tfr_id = TFR_T_RECORD_OFFSET
 
 
+class VectorUDT(DataType):
+    """Spark ML's ``org.apache.spark.ml.linalg.VectorUDT`` (``org.apache.spark.mllib.linalg.VectorUDT`` has the same sqlType and
+    maps to it too).  Read as a dense vector of what an ArrayType(DoubleType) field reads; written as the FloatList of
+    ``toArray`` (include/tfrgpu.h, VECTORS).  Only as a top-level field: ArrayType(VectorUDT) is refused."""
+    tfr_id = TFR_T_VECTOR
+    CLASS_NAMES = ("org.apache.spark.ml.linalg.VectorUDT", "org.apache.spark.mllib.linalg.VectorUDT")
+
+    @staticmethod
+    def sqlType() -> str:
+        return "struct<type:tinyint,size:int,indices:array<int>,values:array<double>>"
+
+
+class DenseVector:
+    """Spark ML's DenseVector: the value type of a VectorUDT field as the reader returns it."""
+
+    def __init__(self, values):
+        self.values = np.asarray(values, dtype=np.float64).reshape(-1)
+
+    @property
+    def size(self) -> int:
+        return len(self.values)
+
+    def toArray(self) -> np.ndarray:
+        return self.values
+
+    def __eq__(self, other):
+        return isinstance(other, (DenseVector, SparseVector)) and np.array_equal(self.toArray(), other.toArray())
+
+    def __len__(self):
+        return self.size
+
+    def __repr__(self):
+        return f"DenseVector({self.values.tolist()!r})"
+
+
+class SparseVector:
+    """Spark ML's SparseVector, with its constructor's checks: size >= 0, as many indices as values, indices strictly
+    increasing inside [0, size)."""
+
+    def __init__(self, size: int, indices, values):
+        self.size = int(size)
+        self.indices = np.asarray(indices, dtype=np.int32).reshape(-1)
+        self.values = np.asarray(values, dtype=np.float64).reshape(-1)
+        if self.size < 0:
+            raise ValueError(f"the size of a sparse vector must be no less than 0, not {self.size}")
+        if len(self.indices) != len(self.values):
+            raise ValueError(f"{len(self.indices)} indices and {len(self.values)} values")
+        if len(self.indices) and (self.indices[0] < 0 or self.indices[-1] >= self.size or np.any(np.diff(self.indices) <= 0)):
+            raise ValueError(f"indices must be strictly increasing and inside [0, {self.size})")
+
+    def toArray(self) -> np.ndarray:
+        out = np.zeros(self.size, dtype=np.float64)
+        out[self.indices] = self.values
+        return out
+
+    def __eq__(self, other):
+        return isinstance(other, (DenseVector, SparseVector)) and np.array_equal(self.toArray(), other.toArray())
+
+    def __len__(self):
+        return self.size
+
+    def __repr__(self):
+        return f"SparseVector({self.size}, {self.indices.tolist()!r}, {self.values.tolist()!r})"
+
+
 class TimestampType(DataType):
     """Exists only so the reference's "unsupported data type" tests can be restated."""
 
@@ -134,7 +202,7 @@ class StructType:
 
 def lower_type(dt: DataType):
     """DataType -> (elem_type_id, depth).  Anything the reference rejects lowers to
-    (TFR_T_UNSUPPORTED, depth) and is refused by tfr_schema_create."""
+    (TFR_T_UNSUPPORTED, depth) and is refused by tfr_schema_create; so is ArrayType(VectorUDT), (TFR_T_VECTOR, depth > 0)."""
     depth = 0
     while isinstance(dt, ArrayType):
         depth += 1
