@@ -70,7 +70,8 @@ enum {
    * and every validity bit set, so every view of a batch (columns, host copy, Arrow, UnsafeRows) reads them as LongType. */
   TFR_T_ROW_INDEX     = 8,  /* the row's entry index in its file                                */
   TFR_T_RECORD_OFFSET = 9,  /* the file offset of the row's entry                               */
-  TFR_T_VECTOR        = 10  /* Spark ML's VectorUDT, read and written as a FloatList (VECTORS below) */
+  TFR_T_VECTOR        = 10, /* Spark ML's VectorUDT, read and written as a FloatList (VECTORS below) */
+  TFR_T_SPARSE_VECTOR = 11  /* Spark ML's VectorUDT, read and written as TF sparse features (SPARSE VECTORS below) */
 };
 /* VECTORS: TFR_T_VECTOR is org.apache.spark.ml.linalg.VectorUDT (and org.apache.spark.mllib.linalg.VectorUDT, which has the
  * same sqlType: struct<type: tinyint not null, size: int, indices: array<int not null>, values: array<double not null>>).
@@ -102,6 +103,48 @@ enum {
  * These rules are restated from Spark's sources (VectorUDT.serialize / deserialize, SparseVector's constructor,
  * UnsafeRowWriter for a nested struct) and are NOT checked against a JVM, like the partition-row and float-bits rules.  */
 
+/* SPARSE VECTORS: TFR_T_SPARSE_VECTOR is the same VectorUDT (the DataSource option vectorFormat=sparse; `dense`, the default,
+ * is TFR_T_VECTOR), stored as the three features tf.io.SparseFeature(index_key = v_indices, value_key = v_values,
+ * dtype = tf.float32, size = N) reads, plus v_size for FixedLenFeature([], tf.int64):
+ *     <name>TFR_SPARSE_INDICES_SUFFIX  Int64List               ArrayType(IntegerType)  the indices of v.toSparse
+ *     <name>TFR_SPARSE_VALUES_SUFFIX   FloatList               ArrayType(DoubleType)   the values of v.toSparse (toFloat)
+ *     <name>TFR_SPARSE_SIZE_SUFFIX     Int64List of one value  IntegerType             v.size
+ * The values feature is not named <name>: a dense-format reader of a sparse file finds <name> absent (null, or
+ * TFR_E_NULL_IN_NONNULL for a non-nullable field) and never reads the non-zeros as a short dense vector; the reverse alike.
+ *   - Lowering : a sparse-vector field IS those three ordinary fields; every semantic follows from theirs.  The values field
+ *              takes the vector's place, name aside, and its nullability; the indices and size fields are nullable and are
+ *              appended after all n_fields of the caller, in field order (indices, size of the first sparse vector, then the
+ *              next's).  tfr_schema_num_fields, tfr_batch_num_columns and the columns tfr_encode takes are n_fields + 2k for k
+ *              sparse vectors: columns [0, n_fields) are the caller's fields (a sparse vector's is its values, list<double>),
+ *              then each sparse vector's indices (list<int32>) and size (int32).  Encoded entries follow the lowered order.
+ *   - Schema : depth 0 only (ArrayType(VectorUDT) is TFR_E_UNSUPPORTED_TYPE naming the field).  Two fields whose feature keys
+ *              collide (a sparse `v` next to a field `v_values`) are TFR_E_INVALID_ARG naming both.  A ByteArray schema ignores
+ *              it like any data field; schema inference never produces it (a sparse file infers as its three plain fields).
+ *   - Read   : the parts read by every rule of their lowered types (kinds, .head for the size, SequenceExample context and
+ *              heads, FAILFAST / DROPMALFORMED / PERMISSIVE, TFR_F_RESYNC, generated fields, the large-record path).  The vector
+ *              is null exactly when its values are.  An error in a part reports the vector's field index (tfr_batch_info
+ *              .error_field, tfr_batch_dropped's `field`); within a record the parts come after every caller field in
+ *              precedence.  The reader does not check sparse structure (sorted indices inside [0, size), equal lengths), as
+ *              Spark's Parquet and ORC readers of a VectorUDT column do not: SparseVector's constructor does, in
+ *              VectorUDT.deserialize.
+ *   - Rows   : tfr_batch_rows (and _with_partition, _async) have the caller's n_fields fields.  A sparse vector's slot is
+ *              (offset << 32) | size of the nested row UnsafeProjection makes of VectorUDT.serialize(SparseVector(size,
+ *              indices, values)): one null word (bit 1: size null, bit 2: indices null), the slots type = 0 (all zero), size
+ *              (the int in the low 4 bytes), indices = (40 << 32) | bytes, values = (o << 32) | bytes, then the indices'
+ *              UnsafeArrayData (int32 elements) and the values' (doubles), each with a zero element null bitset.  A null size or
+ *              indices has a zero slot, and the array behind it moves up.  A null vector has its bit set and a zero slot.
+ *   - Write, tfr_encode_rows / tfr_encode_rows_submit : the row holds the VectorUDT struct, dense or sparse, checked by every
+ *              malformed-struct clause of VECTORS (TFR_E_INVALID_ARG at the same row).  The parts are those of vector.toSparse:
+ *              the entries whose double is != 0.0 (-0.0 and stored zeros dropped, NaN kept; a tiny double may still become 0.0f
+ *              through toFloat), the index of each, and size.  A null vector omits all three, or is TFR_E_NULL_IN_NONNULL in a
+ *              non-nullable field.  A zero vector writes an empty values and indices list and its size.  The output is
+ *              bounded by the input, so no densify limit applies.
+ * These rules are restated from Spark's sources (VectorUDT.serialize, Vector.toSparse, UnsafeRowWriter for a nested struct) and
+ * TensorFlow's tf.io.SparseFeature, and are NOT checked against a JVM or TensorFlow.  */
+#define TFR_SPARSE_INDICES_SUFFIX "_indices"
+#define TFR_SPARSE_VALUES_SUFFIX  "_values"
+#define TFR_SPARSE_SIZE_SUFFIX    "_size"
+
 /* record types: the `recordType` DataSource option (M/TFRecordFileReader.scala:22,69-80) */
 enum { TFR_RT_EXAMPLE = 0, TFR_RT_SEQUENCE_EXAMPLE = 1, TFR_RT_BYTE_ARRAY = 2 };
 
@@ -111,7 +154,7 @@ typedef struct tfr_field {
   const char* name;      /* UTF-8 bytes, not necessarily NUL terminated */
   int32_t     name_len;
   int32_t     elem_type; /* TFR_T_*  */
-  int32_t     depth;     /* 0, 1, 2 (TFR_T_VECTOR: 0) */
+  int32_t     depth;     /* 0, 1, 2 (TFR_T_VECTOR, TFR_T_SPARSE_VECTOR: 0) */
   int32_t     nullable;  /* StructField.nullable */
 } tfr_field;
 
@@ -134,7 +177,7 @@ const char* tfr_last_error(void);
 int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, int32_t record_type,
                           tfr_schema** out);
 void    tfr_schema_destroy(tfr_schema*);
-int32_t tfr_schema_num_fields(const tfr_schema*);
+int32_t tfr_schema_num_fields(const tfr_schema*);   /* lowered: n_fields + 2 per sparse vector (SPARSE VECTORS) */
 
 /* ---- decode: replaces the body of the buildReader closure ---------------------------- */
 /* flags */
@@ -351,7 +394,7 @@ typedef struct tfr_column {
   int64_t  n_values;       /* leaf elements (bytes for STRING/BINARY)                      */
 } tfr_column;
 
-int32_t tfr_batch_num_columns(tfr_batch*);
+int32_t tfr_batch_num_columns(tfr_batch*);   /* tfr_schema_num_fields: a sparse vector adds its indices and size (SPARSE VECTORS) */
 /* device-resident view (zero copy; valid until tfr_batch_release) */
 int32_t tfr_batch_columns(tfr_batch*, tfr_column* out, int32_t n);
 /* copies every buffer to pinned host memory owned by the batch (D2H on the decoder's
@@ -480,7 +523,7 @@ void    tfr_encoder_destroy(tfr_encoder*);
 /* Replaces write(row) for a batch of rows (M/TFRecordOutputWriter.scala:26-38 ->
  * serializeExample M/TFRecordSerializer.scala:20-35 -> toByteArray -> TFRecordWriter.write):
  * columns in the tfr_column layout above (host or device pointers), n = number of schema
- * fields.  Produces the framed bytes of all rows, in row order, byte-identical to what the
+ * fields (tfr_schema_num_fields: a sparse vector adds its indices and size columns, SPARSE VECTORS).  Produces the framed bytes of all rows, in row order, byte-identical to what the
  * reference writer appends to its output stream.  *out_dev is device memory owned by the
  * encoder, valid until the next tfr_encode/destroy.  A null in a non-nullable column is
  * TFR_E_NULL_IN_NONNULL with *error_row set.                                               */

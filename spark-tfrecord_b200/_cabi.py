@@ -10,7 +10,7 @@ import numpy as np
 
 from .sqltypes import (StructType, lower_type, TFR_T_NULL, TFR_T_INT32, TFR_T_INT64, TFR_T_FLOAT32,
                        TFR_T_FLOAT64, TFR_T_DECIMAL, TFR_T_STRING, TFR_T_BINARY, TFR_T_ROW_INDEX, TFR_T_RECORD_OFFSET,
-                       TFR_T_VECTOR)
+                       TFR_T_VECTOR, TFR_T_SPARSE_VECTOR, lowered_schema, sparse_parts, sparse_vector_fields)
 
 TFR_OK = 0
 TFR_E_INVALID_ARG = -1
@@ -68,15 +68,15 @@ _LEAF_DTYPE = {TFR_T_INT32: np.int32, TFR_T_INT64: np.int64, TFR_T_FLOAT32: np.f
                TFR_T_BINARY: np.uint8, TFR_T_NULL: np.uint8}
 
 
-def make_fields(schema: StructType):
-    """StructType -> (ctypes array of tfr_field, keepalive list)."""
+def make_fields(schema: StructType, vector_format: str = "dense"):
+    """StructType -> (ctypes array of tfr_field, keepalive list); VectorUDT fields by vector_format (lower_type)."""
     n = len(schema)
     arr = (tfr_field * max(n, 1))()
     keep = []
     for i, f in enumerate(schema):
         nm = f.name.encode("utf-8") if isinstance(f.name, str) else bytes(f.name)
         keep.append(nm)
-        t, d = lower_type(f.dataType)
+        t, d = lower_type(f.dataType, vector_format)
         arr[i].name = nm
         arr[i].name_len = len(nm)
         arr[i].elem_type = t
@@ -167,11 +167,18 @@ def column_from_ctypes(c: tfr_column) -> HostColumn:
     return HostColumn(c.elem_type, c.depth, n_rows, validity, offsets, values, null_count=c.null_count)
 
 
-def columns_from_rows(schema: StructType, rows: Sequence[Sequence], record_type: int = 0) -> List[HostColumn]:
+def columns_from_rows(schema: StructType, rows: Sequence[Sequence], record_type: int = 0,
+                      vector_format: str = "dense") -> List[HostColumn]:
     """Row-major Python values -> columnar HostColumns (what TFRecordOutputWriter buffers before
     handing a batch to tfr_encode).  Values follow Spark's external types: int, float, str,
-    bytes, list, list of lists, a DenseVector or SparseVector for VectorUDT (its toArray, as a list<double> column);
-    None = null."""
+    bytes, list, list of lists, a DenseVector or SparseVector for VectorUDT (its toArray, as a list<double> column; with
+    vector_format="sparse", the columns of the lowered schema, filled from its toSparse); None = null."""
+    sp = sparse_vector_fields(schema, vector_format)
+    if sp:
+        parts = [[sparse_parts(row[i]) for i in sp] for row in rows]
+        lowered = [tuple(parts[r][sp.index(i)][1] if i in sp else v for i, v in enumerate(row)) +
+                   tuple(x for p in parts[r] for x in (p[0], p[2])) for r, row in enumerate(rows)]
+        return columns_from_rows(lowered_schema(schema, vector_format), lowered, record_type)
     cols = []
     n = len(rows)
     for ci, f in enumerate(schema):

@@ -173,10 +173,13 @@ def _check(rc: int):
 
 
 class Schema:
-    def __init__(self, schema: StructType, record_type: int = 0):
+    def __init__(self, schema: StructType, record_type: int = 0, vector_format: str = "dense"):
+        """`vector_format`: the `vectorFormat` option, how VectorUDT fields are stored (include/tfrgpu.h, VECTORS and SPARSE
+        VECTORS); "sparse" lowers each to three fields (sqltypes.lowered_schema), and the columns follow the lowered schema"""
         self.struct = schema
         self.record_type = record_type
-        fields, self._keep = make_fields(schema)
+        self.vector_format = vector_format
+        fields, self._keep = make_fields(schema, vector_format)
         h = C.c_void_p()
         _check(lib().tfr_schema_create(fields, len(schema), record_type, C.byref(h)))
         self.h = h
@@ -348,10 +351,10 @@ class Batch:
 
 class Decoder:
     def __init__(self, schema: StructType, record_type: int = 0, device: int = 0, flags: int = A.TFR_F_DEFAULT,
-                 corrupt_field: Optional[int] = None):
+                 corrupt_field: Optional[int] = None, vector_format: str = "dense"):
         """`corrupt_field`: with TFR_F_PERMISSIVE in `flags`, the index of the schema field that receives a failing record's
-        payload (a nullable BinaryType column; tfr_decoder_create_permissive)"""
-        self.schema = Schema(schema, record_type)
+        payload (a nullable BinaryType column; tfr_decoder_create_permissive).  `vector_format`: as Schema's."""
+        self.schema = Schema(schema, record_type, vector_format)
         self.ncols = lib().tfr_schema_num_fields(self.schema.h)     # ByteArray: byteArray, then the generated fields
         h = C.c_void_p()
         if corrupt_field is None:
@@ -436,9 +439,9 @@ class Decoder:
 
 
 class Encoder:
-    def __init__(self, schema: StructType, record_type: int = 0, device: int = 0, flags: int = 0):
-        self.schema = Schema(schema, record_type)
-        self.ncols = 1 if record_type == 2 else len(schema)
+    def __init__(self, schema: StructType, record_type: int = 0, device: int = 0, flags: int = 0, vector_format: str = "dense"):
+        self.schema = Schema(schema, record_type, vector_format)
+        self.ncols = 1 if record_type == 2 else lib().tfr_schema_num_fields(self.schema.h)   # (a sparse vector adds two)
         h = C.c_void_p()
         _check(lib().tfr_encoder_create(self.schema.h, device, flags, C.byref(h)))
         self.h = h

@@ -13,6 +13,7 @@
 #include <memory>
 #include <mutex>
 #include <string>
+#include <unordered_set>
 #include <vector>
 
 #include "common.cuh"
@@ -196,11 +197,18 @@ struct tfr_schema {
   int32_t gen_field[2] = {-1, -1};
   bool generated(int32_t f) const { return f >= 0 && (f == gen_field[0] || f == gen_field[1]); }
   bool has_generated() const { return gen_field[0] >= 0 || gen_field[1] >= 0; }
-  // TFR_T_VECTOR fields (include/tfrgpu.h, VECTORS): 1 per such field, else 0.  Lowered to float64 depth-1 fields, so every
-  // parse and encode kernel treats them as ArrayType(DoubleType); only the UnsafeRow kernels (urows.cuh, rows.cuh) read this.
+  // VectorUDT fields (include/tfrgpu.h, VECTORS, SPARSE VECTORS): VK_* per lowered field.  Lowered to ordinary fields (a dense
+  // vector: a float64 list; a sparse one: its values, and its indices and size appended after the caller's n_user fields), so
+  // every parse and encode kernel treats them as those types; only the UnsafeRow kernels (urows.cuh, rows.cuh) read these.
+  // `part`: a sparse vector's indices field (its size field follows); a part's owner; -1 otherwise.
   std::vector<uint8_t> vec;
-  bool vector(int32_t f) const { return f >= 0 && f < (int32_t)vec.size() && vec[f]; }
-  bool has_vector() const { return std::find(vec.begin(), vec.end(), 1) != vec.end(); }
+  std::vector<int32_t> part;
+  int32_t n_user = 0;
+  bool vector(int32_t f) const { return f >= 0 && f < (int32_t)vec.size() && vec[f] == VK_DENSE; }
+  bool sparse(int32_t f) const { return f >= 0 && f < (int32_t)vec.size() && vec[f] == VK_SPARSE; }
+  bool has_vector() const { return std::find(vec.begin(), vec.end(), (uint8_t)VK_DENSE) != vec.end(); }
+  // the caller's field of lowered field f: a sparse vector's part reports its vector
+  int32_t owner(int32_t f) const { return f >= n_user && f < (int32_t)part.size() ? part[f] : f; }
 };
 
 static uint32_t fnv1a(const uint8_t* p, uint32_t n) { uint32_t h = 2166136261u; for (uint32_t i = 0; i < n; ++i) h = (h ^ p[i]) * 16777619u; return h; }
@@ -255,55 +263,78 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
       add_generated(*s, f, std::string(f.name ? f.name : "", (size_t)f.name_len), &rc);
       if (rc) return rc;
     }
-    s->vec.assign(s->fields.size(), 0);
+    s->vec.assign(s->fields.size(), VK_NONE);
+    s->part.assign(s->fields.size(), -1);
+    s->n_user = (int32_t)s->fields.size();
     *out = s.release();
     return TFR_OK;
   }
-  for (int32_t i = 0; i < n_fields; ++i) {
-    const tfr_field& f = fields[i];
-    if (f.name_len < 0 || (f.name_len > 0 && !f.name)) return fail(TFR_E_INVALID_ARG, "bad field name");
-    std::string nm(f.name ? f.name : "", (size_t)f.name_len);
-    int32_t rc = TFR_OK;
-    s->vec.resize(s->fields.size(), 0);
-    if (add_generated(*s, f, nm, &rc)) { if (rc) return rc; continue; }
-    // a VectorUDT field is an ArrayType(DoubleType) field to every kernel but the UnsafeRow ones (VECTORS)
-    const bool vector = f.elem_type == TFR_T_VECTOR;
-    if (vector && f.depth != 0) return fail(TFR_E_UNSUPPORTED_TYPE, "field '" + nm + "': ArrayType(VectorUDT) is not supported");
-    const int32_t et = vector ? TFR_T_FLOAT64 : f.elem_type, depth = vector ? 1 : f.depth;
-    // newFeatureWriter / newFeatureConverter: anything but these types throws (M/TFRecordDeserializer.scala:119-123,
-    // M/TFRecordSerializer.scala:147,151); ArrayType(NullType) falls into the same default branch
-    bool ok_type = et >= TFR_T_NULL && et <= TFR_T_BINARY && depth >= 0 && depth <= 2 && !(et == TFR_T_NULL && depth > 0);
-    if (!ok_type) return fail(TFR_E_UNSUPPORTED_TYPE, "field '" + nm + "': data type is not supported");
+  // one lowered field, appended
+  auto add = [&](const std::string& key, int32_t et, int32_t depth, bool nullable, uint8_t vk, int32_t part) {
     DevField d{};
+    const int32_t idx = (int32_t)s->fields.size();
     d.name_off = (uint32_t)s->names.size();
-    d.name_len = (uint32_t)f.name_len;
-    s->names.insert(s->names.end(), (const uint8_t*)f.name, (const uint8_t*)f.name + f.name_len);
-    d.hash = fnv1a((const uint8_t*)f.name, d.name_len);
-    d.elem_type = (int8_t)et; d.depth = (int8_t)depth; d.nullable = f.nullable ? 1 : 0;
+    d.name_len = (uint32_t)key.size();
+    s->names.insert(s->names.end(), key.begin(), key.end());
+    d.hash = fnv1a((const uint8_t*)key.data(), d.name_len);
+    d.elem_type = (int8_t)et; d.depth = (int8_t)depth; d.nullable = nullable ? 1 : 0;
     d.kind = (int8_t)required_kind(et);
     bool varlen = et == TFR_T_STRING || et == TFR_T_BINARY;
     d.n_levels = (int16_t)(depth + (varlen ? 1 : 0));
     d.dup_next = -1;
     d.width = type_width(et);
     d.fix_slot = -1; d.var_slot = -1; d.cnt_slot = -1;
-    s->vec.push_back(vector ? 1 : 0);
-    if (f.elem_type == TFR_T_NULL) { /* no storage beyond validity */ }
-    else if (d.n_levels == 0) { d.fix_slot = s->n_fix++; s->fix_field.push_back(i); }
-    else { d.var_slot = s->n_var++; d.cnt_slot = s->n_cnt; s->n_cnt += d.n_levels; s->var_field.push_back(i); }
+    if (et == TFR_T_NULL) { /* no storage beyond validity */ }
+    else if (d.n_levels == 0) { d.fix_slot = s->n_fix++; s->fix_field.push_back(idx); }
+    else { d.var_slot = s->n_var++; d.cnt_slot = s->n_cnt; s->n_cnt += d.n_levels; s->var_field.push_back(idx); }
     s->fields.push_back(d);
+    s->vec.push_back(vk);
+    s->part.push_back(part);
+  };
+  std::vector<std::string> user(n_fields);              // the caller's names
+  std::vector<int32_t> sparse;                          // the sparse vectors, in field order
+  for (int32_t i = 0; i < n_fields; ++i) {
+    const tfr_field& f = fields[i];
+    if (f.name_len < 0 || (f.name_len > 0 && !f.name)) return fail(TFR_E_INVALID_ARG, "bad field name");
+    std::string nm(f.name ? f.name : "", (size_t)f.name_len);
+    user[i] = nm;
+    int32_t rc = TFR_OK;
+    if (add_generated(*s, f, nm, &rc)) { if (rc) return rc; s->vec.push_back(VK_NONE); s->part.push_back(-1); continue; }
+    // a VectorUDT field is an ArrayType(DoubleType) field to every kernel but the UnsafeRow ones (VECTORS); a sparse one is
+    // its values field here, and its indices and size fields are appended below (SPARSE VECTORS)
+    const bool vector = f.elem_type == TFR_T_VECTOR, sp = f.elem_type == TFR_T_SPARSE_VECTOR;
+    if ((vector || sp) && f.depth != 0) return fail(TFR_E_UNSUPPORTED_TYPE, "field '" + nm + "': ArrayType(VectorUDT) is not supported");
+    const int32_t et = vector || sp ? TFR_T_FLOAT64 : f.elem_type, depth = vector || sp ? 1 : f.depth;
+    // newFeatureWriter / newFeatureConverter: anything but these types throws (M/TFRecordDeserializer.scala:119-123,
+    // M/TFRecordSerializer.scala:147,151); ArrayType(NullType) falls into the same default branch
+    bool ok_type = et >= TFR_T_NULL && et <= TFR_T_BINARY && depth >= 0 && depth <= 2 && !(et == TFR_T_NULL && depth > 0);
+    if (!ok_type) return fail(TFR_E_UNSUPPORTED_TYPE, "field '" + nm + "': data type is not supported");
+    if (sp) sparse.push_back(i);
+    add(sp ? nm + TFR_SPARSE_VALUES_SUFFIX : nm, et, depth, f.nullable != 0, vector ? VK_DENSE : sp ? VK_SPARSE : VK_NONE, -1);
   }
-  s->vec.resize(s->fields.size(), 0);
+  s->n_user = n_fields;
+  for (int32_t v : sparse) {
+    s->part[v] = (int32_t)s->fields.size();
+    add(user[v] + TFR_SPARSE_INDICES_SUFFIX, TFR_T_INT32, 1, true, VK_INDICES, v);
+    add(user[v] + TFR_SPARSE_SIZE_SUFFIX, TFR_T_INT32, 0, true, VK_SIZE, v);
+  }
   // Spark refuses duplicate column names for file sources before the reader is built
   // (SchemaUtils.checkColumnNameDuplication), so they never reach TFRecordDeserializer
-  size_t hsz = 2; while (hsz < 2 * (size_t)n_fields + 2) hsz <<= 1;
+  if (std::unordered_set<std::string>(user.begin(), user.end()).size() != user.size())
+    return fail(TFR_E_INVALID_ARG, "Found duplicate column(s) in the data schema");
+  // and two fields may not share a feature key, which only a sparse vector's keys can do past the check above
+  const int32_t nl = (int32_t)s->fields.size();
+  auto key = [&](int32_t f) { const DevField& d = s->fields[f]; return std::string((const char*)&s->names[d.name_off], d.name_len); };
+  size_t hsz = 2; while (hsz < 2 * (size_t)nl + 2) hsz <<= 1;
   s->ht.assign(hsz, -1);
-  for (int32_t i = 0; i < n_fields; ++i) {
+  for (int32_t i = 0; i < nl; ++i) {
     const DevField& d = s->fields[i];
     size_t slot = d.hash & (hsz - 1);
     while (s->ht[slot] >= 0) {
-      const DevField& o = s->fields[s->ht[slot]];
+      const int32_t j = s->ht[slot];
+      const DevField& o = s->fields[j];
       if (o.hash == d.hash && o.name_len == d.name_len && memcmp(&s->names[o.name_off], &s->names[d.name_off], d.name_len) == 0)
-        return fail(TFR_E_INVALID_ARG, "Found duplicate column(s) in the data schema");
+        return fail(TFR_E_INVALID_ARG, "fields '" + user[s->owner(j)] + "' and '" + user[s->owner(i)] + "' have the same feature key '" + key(i) + "'");
       slot = (slot + 1) & (hsz - 1);
     }
     s->ht[slot] = i;
@@ -331,11 +362,12 @@ extern "C" int32_t tfr_schema_num_fields(const tfr_schema* s) { return s ? (int3
 // kernels run on non-blocking streams, which nothing orders after the legacy default stream, and `tp` is a local.
 struct DevSchemaBuf {
   DevBuf fields, names, ht, var_field, templates;
-  DevBuf vec;                                             // tfr_schema::vec, for the UnsafeRow kernels of the encoder
+  DevBuf vec, part;                                       // tfr_schema::vec and ::part, for the UnsafeRow kernels of the encoder
   DevBuf tile_consts; uint32_t tile_consts_bytes = 0;     // tile.cuh: per-schema constants in the shared-memory layout
   DevSchema view{};
   const int32_t* d_var_field() const { return (const int32_t*)var_field.p; }
   const uint8_t* d_vec() const { return (const uint8_t*)vec.p; }
+  const int32_t* d_part() const { return (const int32_t*)part.p; }
   const uint8_t* d_tile_consts() const { return (const uint8_t*)tile_consts.p; }
   // `unkeyed`: a field no feature maps to (schema_rehash), which gets no entry template either
   int32_t upload(const tfr_schema& s, cudaStream_t st, int32_t unkeyed = -1) {
@@ -345,8 +377,10 @@ struct DevSchemaBuf {
     CUDA_TRY(ht.alloc(s.ht.size() * sizeof(int32_t)));
     CUDA_TRY(var_field.alloc(std::max<size_t>(1, s.var_field.size()) * sizeof(int32_t)));
     CUDA_TRY(vec.alloc(std::max<size_t>(1, nf)));
+    CUDA_TRY(part.alloc(std::max<size_t>(1, nf) * sizeof(int32_t)));
     if (nf) CUDA_TRY(cudaMemcpyAsync(fields.p, s.fields.data(), nf * sizeof(DevField), cudaMemcpyHostToDevice, st));
     if (!s.vec.empty()) CUDA_TRY(cudaMemcpyAsync(vec.p, s.vec.data(), s.vec.size(), cudaMemcpyHostToDevice, st));
+    if (!s.part.empty()) CUDA_TRY(cudaMemcpyAsync(part.p, s.part.data(), s.part.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     if (!s.names.empty()) CUDA_TRY(cudaMemcpyAsync(names.p, s.names.data(), s.names.size(), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(ht.p, s.ht.data(), s.ht.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     if (!s.var_field.empty()) CUDA_TRY(cudaMemcpyAsync(var_field.p, s.var_field.data(), s.var_field.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));

@@ -319,6 +319,11 @@ struct DevField {
   int32_t width;                             // leaf width in bytes
 };
 
+// What a lowered field is of a VectorUDT (include/tfrgpu.h, VECTORS and SPARSE VECTORS); only the UnsafeRow kernels read it.
+// VK_DENSE: a TFR_T_VECTOR field (a float64 list); VK_SPARSE: a TFR_T_SPARSE_VECTOR's values (a float64 list); VK_INDICES,
+// VK_SIZE: its parts, appended after the caller's fields (an int32 list, an int32).
+enum { VK_NONE = 0, VK_DENSE = 1, VK_SPARSE = 2, VK_INDICES = 3, VK_SIZE = 4 };
+
 struct DevSchema {
   int32_t n_fields, record_type, ht_mask, n_fix, n_var, n_cnt;
   const DevField* fields;

@@ -40,7 +40,9 @@ struct RowsArgs {
   EncCol* cols;                 // [n_fields] the encoder's columns; the layout kernel fills the inner offsets and values
   uint32_t smem_cap;            // tile bytes the shared-memory staging holds
   EncStatus* st;                // rows_first_bad, rows_first_null, rows_overflow, rows_vec_lo / hi
-  const uint8_t* vec;           // [n_fields] 1: a VectorUDT field (a float64 list column filled from the struct)
+  const uint8_t* vec;           // [n_fields] VK_*: VK_DENSE, VK_SPARSE a VectorUDT field (a float64 list column filled from the struct)
+  const int32_t* part;          // [n_fields] VK_SPARSE: the field of its indices (its size's follows)
+  uint32_t nu;                  // the rows' fields: the schema's but a sparse vector's parts, which are filled with it
 };
 
 enum { RW_OK = 0, RW_NULL = 1, RW_BAD = 2 };
@@ -165,15 +167,47 @@ __device__ int rows_vector(const uint8_t* row, uint64_t len, uint64_t slot, bool
   return RW_OK;
 }
 
-// The counts of a field: a vector's level 0 is its dense length.  Its values go to an arena of their own, sized from the
-// scanned counts, so they add nothing to `room`.
+// The counts of a field: a dense-format vector's level 0 is its dense length.  Its values go to an arena of their own, sized
+// from the scanned counts, so they add nothing to `room`.  A sparse-format vector's toSparse entries are counted by pass A
+// itself (rows_sparse_count); they number no more than its stored values, which `room` takes at 8 bytes each, so its values
+// are bounded by the input like a double array's and its int32 indices by half of that (rows_layout sizes the arena so).
 __device__ __forceinline__ int rows_counts(const RowsArgs& A, uint32_t f, const uint8_t* row, uint64_t len, const DevField& fd, uint64_t slot,
                                            uint32_t c[3], uint64_t& room) {
-  if (!A.vec[f]) return rows_field_counts(row, len, fd, slot, c, room);
+  if (A.vec[f] == VK_NONE) return rows_field_counts(row, len, fd, slot, c, room);
   RowsVec v;
   if (rows_vector(row, len, slot, true, v) != RW_OK) return RW_BAD;
   c[0] = v.size;
+  if (A.vec[f] == VK_SPARSE) room += 8ull * v.n;
   return RW_OK;
+}
+
+// toSparse keeps the entries whose double is != 0.0: not +0.0 or -0.0 (a NaN is kept)
+__device__ __forceinline__ bool rows_nz(uint64_t bits) { return (bits << 1) != 0; }
+#define ROWS_VEC_WARP 64u
+// The toSparse entries of a (well-formed) vector at `slot`, and the vector in v; warp-uniform call, `act`: this lane has one.
+// A vector of ROWS_VEC_WARP stored values or more is counted by the whole warp (a dense 2^18-value one is not one lane's scan).
+__device__ __forceinline__ uint32_t rows_sparse_count(const uint8_t* row, uint64_t slot, bool act, RowsVec& v) {
+  const uint32_t lane = threadIdx.x & 31;
+  v = RowsVec{};
+  if (act) rows_vector(row, ~0ull, slot, false, v);
+  const bool big = act && v.n >= ROWS_VEC_WARP;
+  uint32_t k = 0;
+  if (act && !big) for (uint32_t i = 0; i < v.n; ++i) k += rows_nz(rows_ld64(row + v.vals + 8ull * i)) ? 1u : 0u;
+  uint32_t m = __ballot_sync(FULLMASK, big);
+  while (m) {
+    const int l = __ffs(m) - 1;
+    m &= m - 1;
+    const uint8_t* rw = (const uint8_t*)__shfl_sync(FULLMASK, (unsigned long long)row, l);
+    const uint32_t n = __shfl_sync(FULLMASK, v.n, l);
+    const uint64_t vals = __shfl_sync(FULLMASK, v.vals, l);
+    uint32_t t = 0;
+    for (uint32_t i0 = 0; i0 < n; i0 += 32) {
+      const uint32_t i = i0 + lane;
+      t += __popc(__ballot_sync(FULLMASK, i < n && rows_nz(rows_ld64(rw + vals + 8ull * i))));
+    }
+    if (lane == (uint32_t)l) k = t;
+  }
+  return k;
 }
 
 __device__ __forceinline__ bool rows_field_null(const uint8_t* row, uint32_t f) { return (rows_ld64(row + 8ull * (f >> 6)) >> (f & 63)) & 1; }
@@ -212,7 +246,7 @@ __global__ void __launch_bounds__(ROWS_TILE) rows_pass_a_kernel(RowsArgs A) {
   const uint8_t* row = in_tile ? tile_b + (reinterpret_cast<uintptr_t>(A.rows + lo) - g_lo) : A.rows + lo;
 
   // ---- validate ----
-  const uint32_t nf = (uint32_t)A.sch.n_fields, nw = (nf + 63) / 64;
+  const uint32_t nf = A.nu, nw = (nf + 63) / 64;
   bool bad = active && (lo < A.first || hi > A.last || lo > hi || ((lo | hi) & 7) || hi - lo < 8ll * (nw + nf));
   bool nul = false;
   const uint64_t len = (active && !bad) ? (uint64_t)(hi - lo) : 0;
@@ -239,6 +273,17 @@ __global__ void __launch_bounds__(ROWS_TILE) rows_pass_a_kernel(RowsArgs A) {
     const bool present = ok && fd.elem_type != TFR_T_NULL && !rows_field_null(row, f);
     const uint32_t vb = __ballot_sync(FULLMASK, present);
     if (lane == 0) A.valid[(size_t)f * A.vwords + blockIdx.x] = vb;
+    if (A.vec[f] == VK_SPARSE) {                            // its values, and its parts: the indices (as many) and the size
+      RowsVec v;
+      const uint32_t k = rows_sparse_count(row, present ? rows_ld64(row + 8ull * (nw + f)) : 0, present, v);
+      const int32_t pi = A.part[f];
+      if (lane == 0) A.valid[(size_t)pi * A.vwords + blockIdx.x] = A.valid[(size_t)(pi + 1) * A.vwords + blockIdx.x] = vb;
+      if (!active) continue;
+      A.cnt[(size_t)fd.cnt_slot * A.n_rows + r] = k;
+      A.cnt[(size_t)A.sch.fields[pi].cnt_slot * A.n_rows + r] = k;
+      reinterpret_cast<uint32_t*>(A.fixv[pi + 1])[r] = present ? v.size : 0u;
+      continue;
+    }
     if (!active || fd.elem_type == TFR_T_NULL) continue;
     if (fd.n_levels == 0) {
       const uint64_t s = present ? rows_ld64(row + 8ull * (nw + f)) : 0;
@@ -279,7 +324,7 @@ __global__ void rows_layout_kernel(RowsArgs A, const unsigned long long* __restr
     for (uint32_t f = 0; f < nf; ++f) {
       const DevField& fd = A.sch.fields[f];
       if (fd.n_levels == 0) continue;
-      if (A.vec[f]) { xpos = rows_vec_place(xpos, totals[fd.cnt_slot]); xn += totals[fd.cnt_slot]; continue; }
+      if (A.vec[f] == VK_DENSE) { xpos = rows_vec_place(xpos, totals[fd.cnt_slot]); xn += totals[fd.cnt_slot]; continue; }
       for (int l = 1; l < fd.n_levels; ++l) ipos += totals[fd.cnt_slot + l - 1] + 1;
       vpos = ((vpos + 15) & ~15ull) + totals[fd.cnt_slot + fd.n_levels - 1] * (unsigned long long)fd.width;
     }
@@ -290,7 +335,7 @@ __global__ void rows_layout_kernel(RowsArgs A, const unsigned long long* __restr
       for (uint32_t f = 0; f < nf; ++f) {
         const DevField& fd = A.sch.fields[f];
         if (fd.n_levels == 0) continue;
-        if (A.vec[f]) {
+        if (A.vec[f] == VK_DENSE) {
           xpos = (xpos + 15) & ~15ull;
           A.cols[f].values = xarena + xpos;
           xpos = rows_vec_place(xpos, totals[fd.cnt_slot]);
@@ -365,7 +410,6 @@ __device__ __forceinline__ void rows_copy_elems(const DevField& fd, void* values
 // A vector's dense values (toArray) from index 0 of `out`; warp-uniform call, `act`: this lane has a (well-formed) vector.
 // Dense: its lane copies the values, like a double array.  Sparse: a zero-fill of the dense range, then the scatter of the
 // non-zeros; a range of ROWS_VEC_WARP values or more is filled and scattered by the whole warp (HashingTF's are 2^18 long).
-#define ROWS_VEC_WARP 64u
 __device__ __forceinline__ void rows_vector_fill(const uint8_t* row, uint64_t slot, unsigned long long* out, bool act) {
   const uint32_t lane = threadIdx.x & 31;
   RowsVec v{};
@@ -393,6 +437,48 @@ __device__ __forceinline__ void rows_vector_fill(const uint8_t* row, uint64_t sl
   }
 }
 
+// A vector's toSparse (rows_sparse_count's entries): its values to `ov` and their indices to `oi`, from index 0, in index
+// order; warp-uniform call, `act`: this lane has a (well-formed) vector.  ROWS_VEC_WARP stored values or more: the whole warp
+// compacts 32 at a time, each entry placed by the ballot's population below its lane.
+__device__ __forceinline__ void rows_sparse_fill(const uint8_t* row, uint64_t slot, unsigned long long* ov, int32_t* oi, bool act) {
+  const uint32_t lane = threadIdx.x & 31;
+  RowsVec v{};
+  if (act) rows_vector(row, ~0ull, slot, false, v);
+  const bool big = act && v.n >= ROWS_VEC_WARP;
+  if (act && !big) {
+    uint32_t k = 0;
+    for (uint32_t i = 0; i < v.n; ++i) {
+      const uint64_t x = rows_ld64(row + v.vals + 8ull * i);
+      if (!rows_nz(x)) continue;
+      ov[k] = x;
+      oi[k++] = v.sparse ? reinterpret_cast<const int32_t*>(row + v.idx)[i] : (int32_t)i;
+    }
+  }
+  uint32_t m = __ballot_sync(FULLMASK, big);
+  while (m) {
+    const int l = __ffs(m) - 1;
+    m &= m - 1;
+    unsigned long long* o = (unsigned long long*)__shfl_sync(FULLMASK, (unsigned long long)ov, l);
+    int32_t* q = (int32_t*)__shfl_sync(FULLMASK, (unsigned long long)oi, l);
+    const uint8_t* rw = (const uint8_t*)__shfl_sync(FULLMASK, (unsigned long long)row, l);
+    const uint32_t n = __shfl_sync(FULLMASK, v.n, l);
+    const bool sp = __shfl_sync(FULLMASK, v.sparse ? 1 : 0, l) != 0;
+    const uint64_t vals = __shfl_sync(FULLMASK, v.vals, l), idx = __shfl_sync(FULLMASK, v.idx, l);
+    uint32_t base = 0;
+    for (uint32_t i0 = 0; i0 < n; i0 += 32) {
+      const uint32_t i = i0 + lane;
+      const uint64_t x = i < n ? rows_ld64(rw + vals + 8ull * i) : 0;
+      const uint32_t b = __ballot_sync(FULLMASK, rows_nz(x));
+      if (rows_nz(x)) {
+        const uint32_t p = base + __popc(b & ((1u << lane) - 1));
+        o[p] = x;
+        q[p] = sp ? reinterpret_cast<const int32_t*>(rw + idx)[i] : (int32_t)i;
+      }
+      base += __popc(b);
+    }
+  }
+}
+
 __global__ void __launch_bounds__(ROWS_B_WARPS * 32) rows_pass_b_kernel(RowsArgs A) {
   if (A.st->rows_overflow) return;                                   // the columns were not placed: nothing to fill
   const uint32_t lane = threadIdx.x & 31;
@@ -400,7 +486,7 @@ __global__ void __launch_bounds__(ROWS_B_WARPS * 32) rows_pass_b_kernel(RowsArgs
   const uint32_t r = w * 32 + lane;
   if (w * 32 >= A.n_rows) return;                            // warp-uniform
   const bool active = r < A.n_rows;
-  const uint32_t nf = (uint32_t)A.sch.n_fields, nw = (nf + 63) / 64;
+  const uint32_t nf = A.nu, nw = (nf + 63) / 64;
   const uint8_t* row = A.rows + (active ? A.offs[r] : A.first);
   for (uint32_t f = 0; f < nf; ++f) {
     const DevField& fd = A.sch.fields[f];
@@ -412,7 +498,11 @@ __global__ void __launch_bounds__(ROWS_B_WARPS * 32) rows_pass_b_kernel(RowsArgs
     const uint64_t slot = v ? rows_ld64(row + 8ull * (nw + f)) : 0;
     const uint64_t o = slot >> 32, sz = slot & 0xffffffffu;
     const int32_t e0 = v ? A.lev[fd.cnt_slot][r] : 0;
-    if (A.vec[f]) { rows_vector_fill(row, slot, reinterpret_cast<unsigned long long*>(values) + e0, v); continue; }
+    if (A.vec[f] == VK_DENSE) { rows_vector_fill(row, slot, reinterpret_cast<unsigned long long*>(values) + e0, v); continue; }
+    if (A.vec[f] == VK_SPARSE) {
+      rows_sparse_fill(row, slot, reinterpret_cast<unsigned long long*>(values) + e0, (int32_t*)A.cols[A.part[f]].values + e0, v);
+      continue;
+    }
     if (fd.depth == 0) { rows_copy(values + e0, row + o, (uint32_t)sz, v); continue; }
     if (!v) continue;
     const bool var = rows_is_var(fd);

@@ -39,8 +39,10 @@
 #define UROWS_SIZE_THREADS 256
 #define UROWS_BIG 256u
 
-// UR_VEC: a VectorUDT field (include/tfrgpu.h, VECTORS), a float64 list column written as the nested row of a dense vector
-enum { UR_NULL = 0, UR_FIX4 = 1, UR_FIX8 = 2, UR_BYTES = 3, UR_ARR = 4, UR_ARR2 = 5, UR_VEC = 6 };
+// UR_VEC: a VectorUDT field (include/tfrgpu.h, VECTORS), a float64 list column written as the nested row of a dense vector.
+// UR_SVEC: a sparse-vector field (SPARSE VECTORS), its values column written with its indices and size columns (cols[part],
+// cols[part + 1], which are not row fields of their own) as the nested row of a sparse vector.
+enum { UR_NULL = 0, UR_FIX4 = 1, UR_FIX8 = 2, UR_BYTES = 3, UR_ARR = 4, UR_ARR2 = 5, UR_VEC = 6, UR_SVEC = 7 };
 #define UR_VEC_HEAD 40u         // the nested row's fixed part: one null word and four slots
 
 struct UrCol {                  // one decoded column (tfr_column), device pointers
@@ -49,12 +51,12 @@ struct UrCol {                  // one decoded column (tfr_column), device point
   const uint8_t* values;
   int32_t kind;                 // UR_*
   int32_t width;                // leaf bytes of a numeric leaf (4 / 8); 0 for string / binary leaves
-  int32_t var;                  // index among the variable-width fields (UR_BYTES, UR_ARR, UR_ARR2), -1 otherwise
-  int32_t pad;
+  int32_t var;                  // index among the variable-width fields (UR_BYTES, UR_ARR, UR_ARR2, UR_VEC, UR_SVEC), -1 otherwise
+  int32_t part;                 // UR_SVEC: the column of its indices (its size's follows), 0 otherwise
 };
 
 struct UrArgs {
-  const UrCol* cols;            // [nf]
+  const UrCol* cols;            // [nf], then the columns of the sparse vectors' parts
   uint32_t nf, nw, n_rows;      // nw: null words of the full row, (nf + np + 63) / 64
   // the partition values (tfr_batch_rows_with_partition), the same in every row: np slots after the nf data slots, null bit
   // nf + j, and the partition row's variable region (pvw words) at the end of the row.  np = pvw = 0 without them.
@@ -88,20 +90,24 @@ __device__ __forceinline__ uint64_t ur_arr1_bytes(const UrCol& c, int lvl, int64
   for (int64_t j = e0; j < e1; ++j) s += ur_pad8((uint64_t)(o[j + 1] - o[j]));
   return s;
 }
-// the raw size of field c's value in row r (what its slot holds): string / binary length or array bytes
-__device__ __forceinline__ uint64_t ur_value_bytes(const UrCol& c, uint32_t r) {
+__device__ __forceinline__ bool ur_present(const UrCol& c, uint32_t r) {
+  return c.kind != UR_NULL && ((c.valid[r >> 5] >> (r & 31)) & 1u);
+}
+// the raw size of field c's value in row r (what its slot holds): string / binary length, array or nested row bytes
+__device__ __forceinline__ uint64_t ur_value_bytes(const UrCol& c, const UrCol* cols, uint32_t r) {
   const int32_t* o0 = c.off[0];
   const int64_t a = o0[r], b = o0[r + 1];
   if (c.kind == UR_BYTES) return (uint64_t)(b - a);
   if (c.kind == UR_ARR) return ur_arr1_bytes(c, 0, a, b);
   if (c.kind == UR_VEC) return UR_VEC_HEAD + ur_arr1_bytes(c, 0, a, b);
+  if (c.kind == UR_SVEC) {                                  // the indices array (when not null), then the values array
+    const UrCol& ci = cols[c.part];
+    return UR_VEC_HEAD + ur_arr1_bytes(c, 0, a, b) + (ur_present(ci, r) ? ur_arr1_bytes(ci, 0, ci.off[0][r], ci.off[0][r + 1]) : 0);
+  }
   uint64_t s = ur_hdr((uint64_t)(b - a)) + 8 * (uint64_t)(b - a);          // UR_ARR2: steps are inner arrays
   const int32_t* o1 = c.off[1];
   for (int64_t k = a; k < b; ++k) s += ur_arr1_bytes(c, 1, o1[k], o1[k + 1]);
   return s;
-}
-__device__ __forceinline__ bool ur_present(const UrCol& c, uint32_t r) {
-  return c.kind != UR_NULL && ((c.valid[r >> 5] >> (r & 31)) & 1u);
 }
 
 // CAP: launched over the row capacity A.n_rows (the stride of `pos`); rows at or beyond ctl[URC_N] get size 0 and read no column
@@ -120,7 +126,7 @@ __global__ void __launch_bounds__(UROWS_SIZE_THREADS) urows_size_kernel(UrArgs A
     const UrCol& c = A.cols[f];
     if (c.var < 0) continue;
     A.pos[(size_t)c.var * A.n_rows + r] = (uint32_t)s;
-    if (ur_present(c, r)) s += ur_pad8(ur_value_bytes(c, r));
+    if (ur_present(c, r)) s += ur_pad8(ur_value_bytes(c, A.cols, r));
   }
   s += 8ull * A.pvw;
   const bool big = s > 0x7fffffffull;
@@ -156,6 +162,27 @@ __device__ __forceinline__ void ur_vec_head(uint8_t* dst, uint64_t arr) {
   ur_st64(dst, 0x6ull);
   ur_st64(dst + 8, 1ull);
   ur_st64(dst + 32, ((uint64_t)UR_VEC_HEAD << 32) | arr);
+}
+
+// row r's sparse vector of field c at dst (zeroed): the nested row of VectorUDT.serialize(SparseVector(size, indices, values)),
+// its fixed part (null bit 1: size null, bit 2: indices null; type 0; the size; the two array slots) and the arrays' headers by
+// k0 == 0, the elements by k0, k0 + step, ...  (a lane: 0, 1; the whole warp: lane, 32)
+__device__ void ur_emit_svec(const UrCol& c, const UrCol* cols, uint32_t r, uint8_t* dst, uint32_t k0, uint32_t step) {
+  const UrCol& ci = cols[c.part];
+  const UrCol& cs = cols[c.part + 1];
+  const bool ip = ur_present(ci, r), sp = ur_present(cs, r);
+  const int64_t a = c.off[0][r], b = c.off[0][r + 1], ia = ip ? ci.off[0][r] : 0, ib = ip ? ci.off[0][r + 1] : 0;
+  const uint64_t m = (uint64_t)(b - a), mi = (uint64_t)(ib - ia);
+  const uint64_t ibytes = ip ? ur_arr1_bytes(ci, 0, ia, ib) : 0, vo = UR_VEC_HEAD + ibytes;
+  if (k0 == 0) {
+    ur_st64(dst, (sp ? 0ull : 2ull) | (ip ? 0ull : 4ull));
+    if (sp) ur_st64(dst + 16, (uint64_t)reinterpret_cast<const uint32_t*>(cs.values)[r]);
+    if (ip) { ur_st64(dst + 24, ((uint64_t)UR_VEC_HEAD << 32) | ibytes); ur_st64(dst + UR_VEC_HEAD, mi); }
+    ur_st64(dst + 32, (vo << 32) | ur_arr1_bytes(c, 0, a, b));
+    ur_st64(dst + vo, m);
+  }
+  if (ip) ur_copy_elems(dst + UR_VEC_HEAD + ur_hdr(mi), ci.values + (uint64_t)ia * 4, mi, 4, k0, step);
+  ur_copy_elems(dst + vo + ur_hdr(m), c.values + (uint64_t)a * 8, m, 8, k0, step);
 }
 
 // one lane writes the 1-D array of elements [e0, e1) of level lvl + 1 at dst (zeroed); returns its bytes
@@ -283,18 +310,19 @@ __global__ void __launch_bounds__(UROWS_WARPS * 32) urows_emit_kernel(UrArgs A, 
     if (c.var < 0) continue;
     uint64_t len = 0, p = 0;
     if (present) {
-      len = ur_value_bytes(c, r);
+      len = ur_value_bytes(c, A.cols, r);
       p = A.pos[(size_t)c.var * A.n_rows + r];
       ur_st64(slot, (p << 32) | len);
     }
     const bool big = present && ur_pad8(len) >= UROWS_BIG;
-    if (present && !big) ur_emit_lane(c, r, row + p);
+    if (present && !big) { if (c.kind == UR_SVEC) ur_emit_svec(c, A.cols, r, row + p, 0, 1); else ur_emit_lane(c, r, row + p); }
     uint32_t mb = __ballot_sync(FULLMASK, big);
     while (mb) {
       const int l = __ffs(mb) - 1;
       mb &= mb - 1;
       uint8_t* d = (uint8_t*)__shfl_sync(FULLMASK, (unsigned long long)(row + p), l);
-      ur_emit_warp(c, r0 + (uint32_t)l, d);
+      if (c.kind == UR_SVEC) ur_emit_svec(c, A.cols, r0 + (uint32_t)l, d, lane, 32);
+      else ur_emit_warp(c, r0 + (uint32_t)l, d);
     }
   }
   // ---- the partition values: lane = row, warp w takes units w, w + UROWS_WARPS, ... of [the null words holding partition

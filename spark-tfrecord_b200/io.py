@@ -30,7 +30,7 @@ import numpy as np
 from . import _cabi, _native
 from ._cabi import TFR_F_DEFAULT, TFR_F_DROP_MALFORMED, TFR_F_PERMISSIVE, TFR_F_RESYNC, TFR_E_BATCH_TOO_LARGE as A_TFR_E_BATCH_TOO_LARGE, columns_from_rows
 from .sqltypes import (RECORD_TYPES, BinaryType, DenseVector, LongType, RecordOffsetType, RowIndexType, SparseVector, StructField,
-                       StructType, VectorUDT, byte_array_schema)
+                       StructType, VectorUDT, byte_array_schema, check_vector_format, sparse_vector_fields)
 
 M = "src/main/scala/com/linkedin/spark/datasources/tfrecord/"
 _LOG = logging.getLogger(__name__)
@@ -57,6 +57,17 @@ def _record_type(options: Optional[Dict[str, str]]) -> int:
     if rt not in RECORD_TYPES:                                  # :78-79
         raise _native.IllegalArgumentException(-3, f"Unsupported recordType {rt}: recordType can be ByteArray, Example or SequenceExample")
     return RECORD_TYPES[rt]
+
+
+def _vector_format(options: Optional[Dict[str, str]]) -> str:
+    """the `vectorFormat` option: how VectorUDT fields are stored.  "dense" (the default): the FloatList of toArray under the
+    field's name; "sparse": the TF sparse features <name>_indices, <name>_values and <name>_size of toSparse (include/tfrgpu.h,
+    SPARSE VECTORS).  Anything else is refused before any work."""
+    vf = (options or {}).get("vectorFormat", "dense")
+    try:
+        return check_vector_format(vf)
+    except ValueError as e:
+        raise _native.IllegalArgumentException(-1, str(e)) from None
 
 
 def _corrupt_column_name(options: Optional[Dict[str, str]]) -> str:
@@ -229,12 +240,26 @@ def _open_write(path: str, codec: Optional[str]):
     return open(path, "wb")
 
 
-def _rows_of(batch: "_native.Batch", schema: Optional[StructType] = None) -> List[tuple]:
-    """the batch's rows; a VectorUDT field of `schema` (the decoder's, Example or SequenceExample) becomes a DenseVector"""
+def _rows_of(batch: "_native.Batch", schema: Optional[StructType] = None, vector_format: str = "dense") -> List[tuple]:
+    """the batch's rows; a VectorUDT field of `schema` (the decoder's, Example or SequenceExample) becomes a DenseVector, or
+    with vector_format="sparse" a SparseVector of its three lowered columns (null when its values are), whose constructor
+    checks what the decoder does not (SPARSE VECTORS)"""
     cols = batch.to_host()
-    vec = [isinstance(f.dataType, VectorUDT) for f in schema] if schema is not None else [False] * len(cols)
-    return [tuple(DenseVector(v) if (vec[i] and v is not None) else v for i, v in enumerate(c.get(r) for c in cols))
-            for r in range(batch.n_rows)]
+    if schema is None:
+        return [tuple(c.get(r) for c in cols) for r in range(batch.n_rows)]
+    nf = len(schema)
+    sp = {i: nf + 2 * j for j, i in enumerate(sparse_vector_fields(schema, vector_format))}
+    vec = [isinstance(f.dataType, VectorUDT) for f in schema]
+
+    def value(i, r):
+        v = cols[i].get(r)
+        if v is None or not vec[i]:
+            return v
+        if i not in sp:
+            return DenseVector(v)
+        idx, size = cols[sp[i]].get(r), cols[sp[i] + 1].get(r)
+        return SparseVector(0 if size is None else size, [] if idx is None else idx, v)
+    return [tuple(value(i, r) for i in range(nf)) for r in range(batch.n_rows)]
 
 
 class TFRecordDeserializer:
@@ -364,9 +389,10 @@ class TFRecordFileReader:
         metadata columns) holds each row's entry index in the file or the file offset of its entry (in the decompressed
         stream for a compressed file), filled on the GPU.  ByteArray rows are byteArray, then those fields."""
         rt = _record_type(options)
+        vf = _vector_format(options)
         flags, corrupt = _read_mode(options, schema if dataSchema is None else dataSchema, schema)
         block = block_bytes or TFRecordFileReader.BLOCK_BYTES
-        dec = _native.Decoder(_decoder_schema(schema), rt, device, flags, corrupt_field=corrupt)
+        dec = _native.Decoder(_decoder_schema(schema), rt, device, flags, corrupt_field=corrupt, vector_format=vf)
 
         def gen():
             todo = []
@@ -396,7 +422,7 @@ class TFRecordFileReader:
 
                     def drain(batch, block_pos):
                         try:
-                            for row in _rows_of(batch, schema if rt != 2 else None):
+                            for row in _rows_of(batch, schema if rt != 2 else None, vf):
                                 yield row
                             if flags & (TFR_F_DROP_MALFORMED | TFR_F_PERMISSIVE):
                                 dropped = batch.dropped()
@@ -430,8 +456,8 @@ class TFRecordFileReader:
         return gen()
 
 
-def _row_bytes(row) -> int:
-    """rough size of a buffered row's values (what decides when the writer flushes)"""
+def _row_bytes(row, sparse: bool = False) -> int:
+    """rough size of a buffered row's values (what decides when the writer flushes); `sparse`: vectors are written sparse"""
     n = 0
     for v in row:
         if v is None:
@@ -439,7 +465,7 @@ def _row_bytes(row) -> int:
         if isinstance(v, (bytes, bytearray, str)):
             n += len(v) + 8
         elif isinstance(v, (DenseVector, SparseVector)):
-            n += 8 * v.size + 8                                  # written dense (toArray)
+            n += (12 * len(v.values) + 24) if sparse else (8 * v.size + 8)     # written as toSparse, or dense (toArray)
         elif isinstance(v, (list, tuple)):
             n += 8 + sum((len(x) + 8) if isinstance(x, (bytes, bytearray, str)) else (8 * len(x) + 8 if isinstance(x, (list, tuple)) else 8) for x in v)
         else:
@@ -455,7 +481,8 @@ class TFRecordOutputWriter:
         self.path = path
         self.recordType = _record_type(options)                 # validated up front; the reference throws at the first write
         self.schema = byte_array_schema() if self.recordType == 2 else dataSchema
-        self._enc = _native.Encoder(self.schema, self.recordType, device)
+        self.vectorFormat = _vector_format(options)
+        self._enc = _native.Encoder(self.schema, self.recordType, device, vector_format=self.vectorFormat)
         self._rows: List[tuple] = []
         self._bytes = 0
         self._out = _open_write(path, _codec_name((options or {}).get("codec", "")))   # CodecStreams.createOutputStream (:19)
@@ -463,13 +490,13 @@ class TFRecordOutputWriter:
     def write(self, row: Sequence) -> None:
         row = tuple(row)
         self._rows.append(row)
-        self._bytes += _row_bytes(row)
+        self._bytes += _row_bytes(row, self.vectorFormat == "sparse")
         if len(self._rows) >= self.FLUSH_ROWS or self._bytes >= self.FLUSH_BYTES:
             self._flush()
 
     def _encode_rows(self, rows: List[tuple]) -> None:
         try:
-            self._out.write(self._enc.encode(columns_from_rows(self.schema, rows, self.recordType)))
+            self._out.write(self._enc.encode(columns_from_rows(self.schema, rows, self.recordType, self.vectorFormat)))
         except _native.TfrError as e:
             if e.code != A_TFR_E_BATCH_TOO_LARGE or len(rows) < 2:
                 raise
@@ -577,10 +604,12 @@ class DefaultSource:
         """-> PartitionedFile => Iterator[row] (filters are accepted and ignored, :123).  options["mode"]: FAILFAST (default),
         DROPMALFORMED, or PERMISSIVE when `dataSchema` holds the corrupt-record column, checked here, before any file is read."""
         _read_mode(options, dataSchema, requiredSchema)
+        _vector_format(options)
         return lambda file: TFRecordFileReader.readFile(None, options, file, requiredSchema, device, dataSchema=dataSchema)
 
     def prepareWrite(self, options: Dict[str, str], dataSchema: StructType):
         codec = _codec_name((options or {}).get("codec", ""))             # :94-102: the option turns output compression on
+        _vector_format(options)
 
         class _Factory:
             def newInstance(self_inner, path, schema, context=None):

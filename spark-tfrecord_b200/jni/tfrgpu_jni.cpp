@@ -6,6 +6,8 @@
 //   final class TfrGpu {
 //     static native long schemaCreate(String[] names, int[] elemTypes, int[] depths, boolean[] nullable, int recordType);
 //     static native int udtElemType(String udtClassName);   // a UserDefinedType's TFR_T_* by class name (VectorUDT: 10), -1 none
+//     static native int udtElemTypeFormat(String udtClassName, String vectorFormat);   // the same under the vectorFormat option:
+//                                                 // VectorUDT 10 (dense) or 11 (sparse), -1 another UDT, -2 another format
 //     static native void schemaDestroy(long schema);
 //     static native long decoderCreate(long schema, int device, int flags);
 //     static native long decoderCreatePermissive(long schema, int device, int flags, int corruptField);   // mode=PERMISSIVE; -1: no corrupt column
@@ -97,6 +99,25 @@ extern "C" JNIEXPORT jint JNICALL Java_com_linkedin_spark_datasources_tfrecord_T
   const std::string name = u ? u : "";
   if (u) env->ReleaseStringUTFChars(className, u);
   return name == "org.apache.spark.ml.linalg.VectorUDT" || name == "org.apache.spark.mllib.linalg.VectorUDT" ? TFR_T_VECTOR : -1;
+}
+// The element type of a UserDefinedType field under the `vectorFormat` option: both VectorUDTs are TFR_T_VECTOR ("dense", the
+// default) or TFR_T_SPARSE_VECTOR ("sparse", include/tfrgpu.h, SPARSE VECTORS); any other UDT is -1; a format other than these
+// is -2, which the glue refuses before any work, naming the option.
+static int32_t udt_elem_type(const std::string& cls, const std::string& format) {
+  if (format != "dense" && format != "sparse") return -2;
+  if (cls != "org.apache.spark.ml.linalg.VectorUDT" && cls != "org.apache.spark.mllib.linalg.VectorUDT") return -1;
+  return format == "sparse" ? TFR_T_SPARSE_VECTOR : TFR_T_VECTOR;
+}
+extern "C" JNIEXPORT jint JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_udtElemTypeFormat(JNIEnv* env, jclass, jstring className,
+                                                                                                       jstring vectorFormat) {
+  std::string s[2];
+  jstring js[2] = {className, vectorFormat};
+  for (int i = 0; i < 2; ++i) {
+    const char* u = js[i] ? env->GetStringUTFChars(js[i], nullptr) : nullptr;
+    s[i] = u ? u : (i ? "dense" : "");
+    if (u) env->ReleaseStringUTFChars(js[i], u);
+  }
+  return udt_elem_type(s[0], s[1]);
 }
 extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_decoderCreate(JNIEnv* env, jclass, jlong schema, jint device, jint flags) {
   tfr_decoder* d = nullptr;

@@ -16,6 +16,10 @@ import numpy as np
 TFR_T_NULL, TFR_T_INT32, TFR_T_INT64, TFR_T_FLOAT32, TFR_T_FLOAT64, TFR_T_DECIMAL, TFR_T_STRING, TFR_T_BINARY = range(8)
 TFR_T_ROW_INDEX, TFR_T_RECORD_OFFSET = 8, 9          # generated fields: read as LongType, never from a record
 TFR_T_VECTOR = 10                                      # Spark ML's VectorUDT (include/tfrgpu.h, VECTORS)
+TFR_T_SPARSE_VECTOR = 11                               # the same, as TF sparse features (include/tfrgpu.h, SPARSE VECTORS)
+# the feature keys of a sparse vector `v`: v + suffix (TFR_SPARSE_*_SUFFIX of include/tfrgpu.h)
+SPARSE_INDICES_SUFFIX, SPARSE_VALUES_SUFFIX, SPARSE_SIZE_SUFFIX = "_indices", "_values", "_size"
+VECTOR_FORMATS = ("dense", "sparse")                   # the `vectorFormat` DataSource option; dense is the default
 TFR_T_UNSUPPORTED = 99
 TFR_RT_EXAMPLE, TFR_RT_SEQUENCE_EXAMPLE, TFR_RT_BYTE_ARRAY = range(3)
 
@@ -105,6 +109,9 @@ class DenseVector:
     def toArray(self) -> np.ndarray:
         return self.values
 
+    def toSparse(self) -> "SparseVector":
+        return _to_sparse(self.size, np.arange(self.size, dtype=np.int32), self.values)
+
     def __eq__(self, other):
         return isinstance(other, (DenseVector, SparseVector)) and np.array_equal(self.toArray(), other.toArray())
 
@@ -135,6 +142,9 @@ class SparseVector:
         out[self.indices] = self.values
         return out
 
+    def toSparse(self) -> "SparseVector":
+        return _to_sparse(self.size, self.indices, self.values)
+
     def __eq__(self, other):
         return isinstance(other, (DenseVector, SparseVector)) and np.array_equal(self.toArray(), other.toArray())
 
@@ -143,6 +153,12 @@ class SparseVector:
 
     def __repr__(self):
         return f"SparseVector({self.size}, {self.indices.tolist()!r}, {self.values.tolist()!r})"
+
+
+def _to_sparse(size: int, indices: np.ndarray, values: np.ndarray) -> SparseVector:
+    """Vector.toSparse: the entries whose double is != 0.0 (-0.0 and stored zeros dropped, NaN kept), in index order."""
+    keep = values != 0.0
+    return SparseVector(size, indices[keep], values[keep])
 
 
 class TimestampType(DataType):
@@ -200,14 +216,54 @@ class StructType:
         return "StructType(%s)" % ", ".join(f"{f.name}:{f.dataType!r}{'' if f.nullable else ' NOT NULL'}" for f in self.fields)
 
 
-def lower_type(dt: DataType):
+def check_vector_format(vector_format: str) -> str:
+    """the `vectorFormat` option's value, refused (ValueError naming the option) unless it is one of VECTOR_FORMATS"""
+    if vector_format not in VECTOR_FORMATS:
+        raise ValueError(f"vectorFormat must be one of {', '.join(VECTOR_FORMATS)}, not {vector_format!r}")
+    return vector_format
+
+
+def lower_type(dt: DataType, vector_format: str = "dense"):
     """DataType -> (elem_type_id, depth).  Anything the reference rejects lowers to
-    (TFR_T_UNSUPPORTED, depth) and is refused by tfr_schema_create; so is ArrayType(VectorUDT), (TFR_T_VECTOR, depth > 0)."""
+    (TFR_T_UNSUPPORTED, depth) and is refused by tfr_schema_create; so is ArrayType(VectorUDT), (TFR_T_VECTOR, depth > 0).
+    A VectorUDT is TFR_T_VECTOR, or TFR_T_SPARSE_VECTOR with vector_format="sparse"."""
+    check_vector_format(vector_format)
     depth = 0
     while isinstance(dt, ArrayType):
         depth += 1
         dt = dt.elementType
+    if dt.tfr_id == TFR_T_VECTOR and vector_format == "sparse":
+        return TFR_T_SPARSE_VECTOR, depth
     return dt.tfr_id, depth
+
+
+def sparse_vector_fields(schema: StructType, vector_format: str = "dense") -> List[int]:
+    """the indexes of the top-level fields that are sparse vectors under vector_format, in field order"""
+    check_vector_format(vector_format)
+    return [i for i, f in enumerate(schema) if vector_format == "sparse" and isinstance(f.dataType, VectorUDT)]
+
+
+def lowered_schema(schema: StructType, vector_format: str = "dense") -> StructType:
+    """The schema every kernel sees (include/tfrgpu.h, SPARSE VECTORS): a sparse vector `v` is its values field
+    v_values: ArrayType(DoubleType) in its place, with its nullability, and the nullable fields v_indices: ArrayType(IntegerType)
+    and v_size: IntegerType appended after all the fields, in field order.  Its columns are the decoder's and the encoder's."""
+    sp = set(sparse_vector_fields(schema, vector_format))
+    out = [StructField(f.name + SPARSE_VALUES_SUFFIX, ArrayType(DoubleType()), f.nullable) if i in sp else f
+           for i, f in enumerate(schema)]
+    for i in sorted(sp):
+        nm = schema[i].name
+        out.append(StructField(nm + SPARSE_INDICES_SUFFIX, ArrayType(IntegerType()), True))
+        out.append(StructField(nm + SPARSE_SIZE_SUFFIX, IntegerType(), True))
+    return StructType(out)
+
+
+def sparse_parts(v):
+    """A vector (DenseVector or SparseVector, or None) -> the values of its three lowered fields, (indices, values, size) of
+    v.toSparse, or (None, None, None) for a null vector."""
+    if v is None:
+        return None, None, None
+    s = v.toSparse()
+    return s.indices.tolist(), s.values.tolist(), int(s.size)
 
 
 # TensorFlowInferSchema.getSchemaForByteArray (M/TensorFlowInferSchema.scala:60-64)
