@@ -48,8 +48,9 @@ enum {
   TFR_E_KIND_MISMATCH    = -15, /* require(...) M/TFRecordDeserializer.scala:178,189,201,212 -> IllegalArgumentException */
   TFR_E_EMPTY_SCALAR     = -16, /* .head on empty list M/TFRecordDeserializer.scala:75-94 -> NoSuchElementException */
   TFR_E_NULL_IN_NONNULL  = -17, /* M/TFRecordDeserializer.scala:31,56 ; M/TFRecordSerializer.scala:29-31,53-55 -> NullPointerException */
-  TFR_E_BAD_NESTING      = -18  /* 2-D column fed from context / scalar column fed from feature_lists:
+  TFR_E_BAD_NESTING      = -18, /* 2-D column fed from context / scalar column fed from feature_lists:
                                    M/TFRecordDeserializer.scala:119,142 -> RuntimeException */
+  TFR_E_INDEX_MISMATCH   = -19  /* a record index that does not describe its file (RECORD INDEX below) -> IOException */
 };
 
 /* ---- schema -------------------------------------------------------------------------- */
@@ -663,6 +664,53 @@ int32_t tfr_infer_skipped(tfr_infer*, int64_t* n_skipped, int64_t* record, int64
 int32_t tfr_infer_result(tfr_infer*, int32_t* n_names);
 int32_t tfr_infer_name(tfr_infer*, int32_t i, const char** name, int32_t* name_len, int32_t* code);
 void    tfr_infer_destroy(tfr_infer*);
+
+/* ---- record index: split large files across tasks ----------------------------------------
+ * RECORD INDEX: a sidecar that lets a reader start at a record boundary anywhere in an uncompressed TFRecord file and know
+ * the entry number there, so a file can be read in splits (the DataSource option recordIndex=true).  A scan for the next
+ * boundary is not safe: a payload can hold a complete, CRC-valid frame.  For data file dir/name the index is
+ * dir/_name.tfrindex (Spark's file listing skips names that start with `_`; restated from Spark's sources, not checked
+ * against a JVM).  All fields are little-endian:
+ *   - a 32-byte header: the magic TFR_INDEX_MAGIC (8 bytes), u64 data_bytes (the data file's size), u64 n_entries (its
+ *     frames) and u64 stride (a power of two, at least 16);
+ *   - then K = ceil(data_bytes / stride) checkpoints of 16 bytes (K = 0 for an empty file).  Checkpoint k is (u64 offset,
+ *     u64 entry) of the first frame whose header offset is >= k * stride; when there is no such frame it is
+ *     (data_bytes, n_entries).
+ * Building.  tfr_index_update streams a file in blocks with the tfr_infer_update_block contract (is_final, *consumed, a
+ * partial frame of a non-final block carried into the next one; blocks below 2 GiB).  Each block runs the frame index
+ * (frame.cuh, every length CRC verified), then index_checkpoint_kernel (index.cuh): one thread per frame, frame i writing the
+ * slots k with o[i-1] < k * stride <= o[i].  A framing error (TFR_E_CRC_LENGTH, TFR_E_TRUNCATED, TFR_E_RECORD_TOO_LARGE) fails
+ * the call with its file offset in tfr_last_error, and every later update and result call returns it: a damaged file gets
+ * no index.  Payload CRCs and protobuf validity are not checked: those are record errors, which a reader's mode handles.
+ * tfr_index_result returns the index bytes (owned by the handle, valid until destroy) once the final block is in.
+ * Seeking.  tfr_index_seek takes bytes that start at a frame boundary (a checkpoint: entry base_entry at file offset
+ * base_offset) and returns the first frame whose header offset is >= target, and its entry number:
+ *   - target <= base_offset: the base itself, with no device work;
+ *   - otherwise the frames are walked with the frame index, their length CRCs verified.  The bytes must reach target + 12
+ *     or the end of the file (TFR_E_INVALID_ARG when they end more than one header before target): at most stride bytes
+ *     plus one header from the checkpoint of floor(target / stride);
+ *   - when the frame in front of target runs past the bytes given, its end is computed from its verified header;
+ *   - when the bytes end (0..7 bytes after the last frame, as at a clean end of file) before target, the result is the end
+ *     of the bytes and the frames before it: the index's (data_bytes, n_entries) when the bytes reach the file's end;
+ *   - a length CRC that fails, a length above 2^31 - 1, a cut-off header or a frame that ends before target although the
+ *     bytes end inside it is TFR_E_INDEX_MISMATCH, with the file offset in tfr_last_error.
+ * A reader of the split [s, e) delivers exactly the frames whose header offset o has s <= o < e: it seeks s and e (e >=
+ * data_bytes is the end of the file) and reads [offset(s), offset(e)) with tfr_decode_submit_at(entry(s), offset(s)), its last
+ * block final.  When the split is read to its end with a different number of entries than entry(e) - entry(s), it fails with
+ * TFR_E_INDEX_MISMATCH before any row of it is handed out.  Compressed files and TFR_F_RESYNC reads are not split.        */
+#define TFR_INDEX_MAGIC            "TFRIDX01"
+#define TFR_INDEX_HEADER_BYTES     32
+#define TFR_INDEX_CHECKPOINT_BYTES 16
+#define TFR_INDEX_MIN_STRIDE       16ull
+#define TFR_INDEX_MAX_STRIDE       (1ull << 30)
+typedef struct tfr_indexer tfr_indexer;
+/* stride: a power of two from TFR_INDEX_MIN_STRIDE to TFR_INDEX_MAX_STRIDE, or TFR_E_INVALID_ARG before any device work */
+int32_t tfr_indexer_create(int32_t device, uint64_t stride, tfr_indexer** out);
+int32_t tfr_index_update(tfr_indexer*, const void* data, size_t nbytes, int32_t on_device, int32_t is_final, size_t* consumed);
+int32_t tfr_index_result(tfr_indexer*, const void** bytes, size_t* nbytes);
+int32_t tfr_index_seek(tfr_indexer*, const void* data, size_t nbytes, int32_t on_device, int64_t base_entry, int64_t base_offset,
+                       int64_t target, int64_t* entry, int64_t* offset);
+void    tfr_indexer_destroy(tfr_indexer*);
 
 #ifdef __cplusplus
 }

@@ -28,6 +28,7 @@ TFR_E_KIND_MISMATCH = -15
 TFR_E_EMPTY_SCALAR = -16
 TFR_E_NULL_IN_NONNULL = -17
 TFR_E_BAD_NESTING = -18
+TFR_E_INDEX_MISMATCH = -19     # a record index that does not describe its file (include/tfrgpu.h, RECORD INDEX)
 
 TFR_F_VERIFY_CRC = 0x1
 TFR_F_DROP_MALFORMED = 0x2       # mode=DROPMALFORMED: failing records are dropped, framing errors still end the block

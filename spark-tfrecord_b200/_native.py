@@ -31,6 +31,7 @@ EXPORTS = [
     "tfr_encoded_result", "tfr_encoded_release", "tfr_encoder_get_stats",
     "tfr_infer_create", "tfr_infer_create_mode", "tfr_infer_update", "tfr_infer_update_block", "tfr_infer_skipped",
     "tfr_infer_result", "tfr_infer_name", "tfr_infer_destroy",
+    "tfr_indexer_create", "tfr_index_update", "tfr_index_result", "tfr_index_seek", "tfr_indexer_destroy",
 ]
 
 
@@ -79,7 +80,7 @@ _EXC = {
     A.TFR_E_KIND_MISMATCH: IllegalArgumentException, A.TFR_E_BAD_RECORD_TYPE: IllegalArgumentException,
     A.TFR_E_EMPTY_SCALAR: NoSuchElementException, A.TFR_E_NULL_IN_NONNULL: NullPointerException,
     A.TFR_E_UNSUPPORTED_TYPE: UnsupportedTypeException, A.TFR_E_BAD_NESTING: UnsupportedTypeException,
-    A.TFR_E_CUDA: CudaError,
+    A.TFR_E_CUDA: CudaError, A.TFR_E_INDEX_MISMATCH: IOException,
 }
 
 
@@ -157,6 +158,11 @@ def lib():
         "tfr_infer_result": (i32, [vp, P(i32)]),
         "tfr_infer_name": (i32, [vp, i32, P(C.c_char_p), P(i32), P(i32)]),
         "tfr_infer_destroy": (None, [vp]),
+        "tfr_indexer_create": (i32, [i32, C.c_uint64, P(vp)]),
+        "tfr_index_update": (i32, [vp, vp, sz, i32, i32, P(sz)]),
+        "tfr_index_result": (i32, [vp, P(vp), P(sz)]),
+        "tfr_index_seek": (i32, [vp, vp, sz, i32, i64, i64, i64, P(i64), P(i64)]),
+        "tfr_indexer_destroy": (None, [vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -653,6 +659,50 @@ class Infer:
     def close(self):
         if self.h:
             lib().tfr_infer_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Indexer:
+    """The record index of one file (tfr_indexer_*, include/tfrgpu.h RECORD INDEX): update() streams the file's framed bytes
+    in blocks, result() is the index once the final block is in.  seek() finds the first frame at or after a file offset
+    from bytes that start at a checkpoint."""
+
+    def __init__(self, stride: int, device: int = 0):
+        h = C.c_void_p()
+        self.h = None
+        _check(lib().tfr_indexer_create(device, stride, C.byref(h)))
+        self.h = h
+
+    def update(self, data, is_final: bool, nbytes: Optional[int] = None) -> int:
+        """one block (host bytes / numpy, a torch tensor, or (ptr, nbytes, on_device)) -> consumed bytes"""
+        ptr, n, on_dev, keep = _device_ptr(data)
+        if nbytes is not None:
+            n = nbytes
+        used = C.c_size_t()
+        _check(lib().tfr_index_update(self.h, ptr, n, on_dev, 1 if is_final else 0, C.byref(used)))
+        return used.value
+
+    def result(self) -> bytes:
+        p, n = C.c_void_p(), C.c_size_t()
+        _check(lib().tfr_index_result(self.h, C.byref(p), C.byref(n)))
+        return C.string_at(p, n.value)
+
+    def seek(self, data, base_entry: int, base_offset: int, target: int) -> tuple:
+        """-> (entry, offset) of the first frame whose header offset is >= target (tfr_index_seek)"""
+        ptr, n, on_dev, keep = _device_ptr(data)
+        e, o = C.c_int64(), C.c_int64()
+        _check(lib().tfr_index_seek(self.h, ptr, n, on_dev, base_entry, base_offset, target, C.byref(e), C.byref(o)))
+        return e.value, o.value
+
+    def close(self):
+        if self.h:
+            lib().tfr_indexer_destroy(self.h)
             self.h = None
 
     def __del__(self):

@@ -24,6 +24,7 @@
 #include "bytes_tile.cuh"
 #include "frame.cuh"
 #include "host_util.h"
+#include "index.cuh"
 #include "infer.cuh"
 #include "large.cuh"
 #include "permissive.cuh"
@@ -79,6 +80,7 @@ extern "C" const char* tfr_status_string(int32_t s) {
     case TFR_E_EMPTY_SCALAR: return "head of empty list";
     case TFR_E_NULL_IN_NONNULL: return "field does not allow null values";
     case TFR_E_BAD_NESTING: return "Cannot convert Feature/FeatureList to this array nesting";
+    case TFR_E_INDEX_MISMATCH: return "record index does not describe its file";
     default: return "unknown status";
   }
 }
@@ -450,6 +452,7 @@ static cudaError_t raise_dyn_smem(size_t smem) {
 }
 
 #include "api_frames.inc"
+#include "api_index.inc"
 #include "api_infer.inc"
 #include "api_outputs.inc"
 #include "api_decode.inc"

@@ -101,6 +101,22 @@ def _resync_flag(options: Optional[Dict[str, str]], mode: str) -> int:
     return TFR_F_RESYNC
 
 
+def _record_index(options: Optional[Dict[str, str]]) -> bool:
+    """the `recordIndex` option ("false" by default, or "true", case-insensitive): the writer puts a record index next to each
+    data file, and the reader splits files that have one (include/tfrgpu.h, RECORD INDEX).  Anything else is refused."""
+    value = (options or {}).get("recordIndex", "false")
+    v = value.lower() if isinstance(value, str) else value
+    if v not in ("true", "false"):
+        raise _native.IllegalArgumentException(-1, f"recordIndex {value}: the option takes true or false")
+    return v == "true"
+
+
+def _check_record_index(options: Optional[Dict[str, str]], codec: Optional[str]) -> None:
+    """recordIndex=true with a codec is refused: a compressed stream cannot be split"""
+    if _record_index(options) and codec:
+        raise _native.IllegalArgumentException(-1, f"recordIndex=true with codec {codec}: a compressed file cannot be split")
+
+
 _MODE_FLAGS = {"FAILFAST": TFR_F_DEFAULT, "DROPMALFORMED": TFR_F_DEFAULT | TFR_F_DROP_MALFORMED, "PERMISSIVE": TFR_F_DEFAULT | TFR_F_PERMISSIVE}
 
 
@@ -238,6 +254,70 @@ def _open_write(path: str, codec: Optional[str]):
     if codec == "deflate":
         return _DeflateWriter(open(path, "wb"))
     return open(path, "wb")
+
+
+# ---- the record index (include/tfrgpu.h, RECORD INDEX) -------------------------------------------------------------------
+RECORD_INDEX_STRIDE = 1 << 20          # what the writer and buildIndex use: 16 bytes of index per MiB of data
+_INDEX_MAGIC = b"TFRIDX01"
+_INDEX_HEADER = struct.Struct("<8sQQQ")
+
+
+def index_path(path: str) -> str:
+    """dir/name -> dir/_name.tfrindex: the leading underscore keeps Spark's file listing from reading it as data"""
+    d, name = os.path.split(path)
+    return os.path.join(d, "_" + name + ".tfrindex")
+
+
+def _index_mismatch(msg: str) -> "_native.TfrError":
+    return _native.error_for(_cabi.TFR_E_INDEX_MISMATCH, f"record index does not describe its file: {msg}")
+
+
+def parse_index(raw: bytes, data_bytes: int):
+    """the index bytes of a data file of `data_bytes` bytes -> (n_entries, stride, checkpoints: uint64 array [K, 2] of
+    (offset, entry)).  A bad magic or stride, another data size, or a length other than 32 + 16 * ceil(data_bytes / stride)
+    raises IOException (TFR_E_INDEX_MISMATCH)."""
+    if len(raw) < _INDEX_HEADER.size:
+        raise _index_mismatch(f"{len(raw)} bytes, shorter than the header")
+    magic, size, n_entries, stride = _INDEX_HEADER.unpack_from(raw)
+    if magic != _INDEX_MAGIC:
+        raise _index_mismatch(f"magic {magic!r}")
+    if stride < 16 or stride & (stride - 1):
+        raise _index_mismatch(f"stride {stride} is not a power of two of at least 16")
+    if size != data_bytes:
+        raise _index_mismatch(f"it describes {size} bytes, the file has {data_bytes}")
+    k = -(-size // stride)
+    if len(raw) != _INDEX_HEADER.size + 16 * k:
+        raise _index_mismatch(f"{len(raw)} bytes, not the header and {k} checkpoints")
+    return n_entries, stride, np.frombuffer(raw, dtype="<u8", offset=_INDEX_HEADER.size).reshape(k, 2)
+
+
+def _read_index(path: str):
+    with open(index_path(path), "rb") as f:
+        return parse_index(f.read(), os.path.getsize(path))
+
+
+def _split_bounds(file: "PartitionedFile", device: int):
+    """(entry, offset) of the first frame at or after the split's start and of the first at or after its end: the split
+    [s, e) delivers the frames whose header offset is in it.  Each is a checkpoint plus tfr_index_seek over at most one
+    stride and one header of the file."""
+    path = file.toPath()
+    size = os.path.getsize(path)
+    n_entries, stride, ck = _read_index(path)
+    idx = _native.Indexer(stride, device)
+    try:
+        with open(path, "rb") as f:
+            def seek(t):
+                if t >= size:
+                    return n_entries, size
+                off, ent = int(ck[t // stride][0]), int(ck[t // stride][1])
+                if off > size or ent > n_entries:
+                    raise _index_mismatch(f"checkpoint {t // stride} ({off}, {ent}) lies past the file's end")
+                f.seek(off)
+                data = f.read(max(0, min(size, t + 12) - off))
+                return idx.seek(data, ent, off, t)
+            return seek(file.start) + seek(file.start + file.length)
+    finally:
+        idx.close()
 
 
 def _rows_of(batch: "_native.Batch", schema: Optional[StructType] = None, vector_format: str = "dense") -> List[tuple]:
@@ -392,29 +472,40 @@ class TFRecordFileReader:
         vf = _vector_format(options)
         flags, corrupt = _read_mode(options, schema if dataSchema is None else dataSchema, schema)
         block = block_bytes or TFRecordFileReader.BLOCK_BYTES
+        # recordIndex=true: a split of a file reads exactly the frames whose header offset lies in it (RECORD INDEX)
+        split = (_record_index(options) and _codec_of_path(file.toPath()) is None
+                 and (file.start, file.length) != (0, os.path.getsize(file.toPath())))
         dec = _native.Decoder(_decoder_schema(schema), rt, device, flags, corrupt_field=corrupt, vector_format=vf)
 
         def gen():
             todo = []
             try:
                 compressed = _codec_of_path(file.toPath()) is not None
+                if split:
+                    ent_s, off_s, ent_e, off_e = _split_bounds(file, device)
                 with _open_read(file.toPath()) as f:
                     if not compressed:
-                        f.seek(file.start)
-                    remaining = (1 << 62) if compressed else file.length          # a compressed file is read to its end
+                        f.seek(off_s if split else file.start)
+                    remaining = (1 << 62) if compressed else off_e - off_s if split else file.length   # a compressed file is read to its end
                     n_slots = dec.num_staging_slots()
                     turn = [0]
-                    pos = [0 if compressed else file.start]     # where the next block starts in the (decompressed) file
-                    entries = [0]                               # and the entries in front of it (the file is read whole)
+                    pos = [off_s if split else 0 if compressed else file.start]   # where the next block starts in the (decompressed) file
+                    entries = [ent_s if split else 0]           # and the entries in front of it
+                    in_slot = {}                                # a split's batch by the staging slot it was read from
 
                     def stage(nbytes):
-                        st = dec.staging_slot(turn[0] % n_slots, nbytes)
+                        slot = turn[0] % n_slots
+                        if slot in in_slot:                     # a split holds its batches until it is checked: the slot's
+                            in_slot.pop(slot).wait()            # batch is done with its input before the slot is refilled
+                        st = dec.staging_slot(slot, nbytes)
                         turn[0] += 1
                         return st
 
                     def process(st, nbytes, final):
                         batch = dec.submit(st, is_final=final, nbytes=nbytes, first_entry=entries[0], first_offset=pos[0])
                         todo.append((batch, pos[0]))
+                        if split:
+                            in_slot[(turn[0] - 1) % n_slots] = batch
                         used, n = batch.extent()
                         pos[0] += used
                         entries[0] += n
@@ -444,8 +535,18 @@ class TFRecordFileReader:
                             batch.release()
 
                     for _ in _stream_blocks(f, remaining, block, stage, process):
-                        while len(todo) > 1:                 # the block before the one just submitted
+                        while len(todo) > 1 and not split:   # the block before the one just submitted
                             yield from drain(*todo.pop(0))
+                    if split:
+                        # the whole file's framing was verified when the index was built: a framing error, or another
+                        # number of entries than the index's, means the index does not describe the file.  Checked before
+                        # any row of the split is handed out.  (A FAILFAST split that stops at a failing record raises
+                        # that record's error after the rows in front of it, as a whole-file read does.)
+                        if any(b.info["error_code"] in _cabi.FRAMING_ERRORS for b, _ in todo):
+                            raise _index_mismatch(f"{file.toPath()}: a framing error inside [{off_s}, {off_e})")
+                        if pos[0] == off_e and entries[0] != ent_e:
+                            raise _index_mismatch(f"{file.toPath()}: {entries[0] - ent_s} entries in [{off_s}, {off_e}), the "
+                                                  f"index says {ent_e - ent_s}")
                     while todo:
                         yield from drain(*todo.pop(0))
             finally:
@@ -485,7 +586,11 @@ class TFRecordOutputWriter:
         self._enc = _native.Encoder(self.schema, self.recordType, device, vector_format=self.vectorFormat)
         self._rows: List[tuple] = []
         self._bytes = 0
-        self._out = _open_write(path, _codec_name((options or {}).get("codec", "")))   # CodecStreams.createOutputStream (:19)
+        codec = _codec_name((options or {}).get("codec", ""))
+        _check_record_index(options, codec)
+        # recordIndex=true: the framed output of every flush is indexed on the GPU from the encoder's device result
+        self._index = _native.Indexer(RECORD_INDEX_STRIDE, device) if _record_index(options) else None
+        self._out = _open_write(path, codec)   # CodecStreams.createOutputStream (:19)
 
     def write(self, row: Sequence) -> None:
         row = tuple(row)
@@ -496,7 +601,12 @@ class TFRecordOutputWriter:
 
     def _encode_rows(self, rows: List[tuple]) -> None:
         try:
-            self._out.write(self._enc.encode(columns_from_rows(self.schema, rows, self.recordType, self.vectorFormat)))
+            cols = columns_from_rows(self.schema, rows, self.recordType, self.vectorFormat)
+            ptr, n = self._enc.encode_columns([c.to_ctypes() for c in cols], False)
+            framed = self._enc.result_host()                     # (waits for the encode: the device bytes are complete)
+            if self._index is not None:
+                self._index.update((ptr, n, 1), False)
+            self._out.write(framed)
         except _native.TfrError as e:
             if e.code != A_TFR_E_BATCH_TOO_LARGE or len(rows) < 2:
                 raise
@@ -510,11 +620,22 @@ class TFRecordOutputWriter:
             self._encode_rows(rows)
 
     def close(self) -> None:
+        """flushes the rows and closes the file; with recordIndex=true then writes its index (a failed write gets none)"""
+        written = False
         try:
             self._flush()
+            written = True
         finally:
             self._out.close()
             self._enc.close()
+            if self._index is not None:
+                try:
+                    if written:
+                        self._index.update(b"", True)
+                        with open(index_path(self.path), "wb") as f:
+                            f.write(self._index.result())
+                finally:
+                    self._index.close()
 
 
 class DefaultSource:
@@ -523,8 +644,50 @@ class DefaultSource:
     def shortName(self) -> str:
         return "tfrecord"
 
-    def isSplitable(self, *a, **k) -> bool:
-        return False                                             # :26-29; splitting happens inside the native side
+    def isSplitable(self, options: Optional[Dict[str, str]] = None, path: Optional[str] = None) -> bool:
+        """False, as in the reference (:26-29), unless recordIndex=true, the file is uncompressed, resyncFraming is not
+        true (a lost region has no place in an index) and the file has an index (_name.tfrindex) whose magic is valid and
+        whose data size is the file's.  Then readFile reads each split [start, start + length) through the index."""
+        if options is None or path is None:
+            return False
+        resync = options.get("resyncFraming", "false")
+        if str(options.get("recordIndex", "false")).lower() != "true" or _codec_of_path(path) is not None or str(resync).lower() == "true":
+            return False
+        try:
+            with open(index_path(path), "rb") as f:
+                head = f.read(_INDEX_HEADER.size)
+        except OSError:
+            return False
+        if len(head) < _INDEX_HEADER.size:
+            return False
+        magic, size, _, _ = _INDEX_HEADER.unpack(head)
+        return magic == _INDEX_MAGIC and size == os.path.getsize(path)
+
+    def buildIndex(self, path: str, stride: int = RECORD_INDEX_STRIDE, device: int = 0) -> str:
+        """writes the record index of an existing uncompressed TFRecord file (one written by TensorFlow, say), streamed
+        through tfr_index_update, and returns its path.  A framing error raises its IOException, and no index is written."""
+        if _codec_of_path(path) is not None:
+            raise _native.IllegalArgumentException(-1, f"{path}: a compressed file cannot be split, so it gets no record index")
+        idx = _native.Indexer(stride, device)
+        buf = [np.empty(0, dtype=np.uint8)]
+
+        def stage(nbytes):
+            if len(buf[0]) < nbytes:
+                buf[0] = np.empty(nbytes + nbytes // 8, dtype=np.uint8)
+            return buf[0]
+
+        try:
+            with open(path, "rb") as f:
+                for _ in _stream_blocks(f, os.path.getsize(path), TFRecordFileReader.BLOCK_BYTES, stage,
+                                        lambda st, nb, final: idx.update(st, final, nb)):
+                    pass
+            raw = idx.result()
+        finally:
+            idx.close()
+        out = index_path(path)
+        with open(out, "wb") as f:
+            f.write(raw)
+        return out
 
     def metadataSchemaFields(self) -> List[Tuple[str, str, "LongType"]]:
         """The generated metadata fields this source fills, as FileFormat.metadataSchemaFields lists them (Spark 3.4 / 3.5:
@@ -605,11 +768,13 @@ class DefaultSource:
         DROPMALFORMED, or PERMISSIVE when `dataSchema` holds the corrupt-record column, checked here, before any file is read."""
         _read_mode(options, dataSchema, requiredSchema)
         _vector_format(options)
+        _record_index(options)
         return lambda file: TFRecordFileReader.readFile(None, options, file, requiredSchema, device, dataSchema=dataSchema)
 
     def prepareWrite(self, options: Dict[str, str], dataSchema: StructType):
         codec = _codec_name((options or {}).get("codec", ""))             # :94-102: the option turns output compression on
         _vector_format(options)
+        _check_record_index(options, codec)
 
         class _Factory:
             def newInstance(self_inner, path, schema, context=None):

@@ -49,6 +49,11 @@
 //     static native long inferUpdate(long infer, java.nio.ByteBuffer block, long nbytes, boolean isFinal);   // -> consumed bytes
 //     static native Object[] inferResult(long infer);     // {String[] names (bytewise sorted), int[] lattice codes}
 //     static native void inferDestroy(long infer);
+//     static native long indexerCreate(int device, long stride);                                 // the record index (recordIndex=true)
+//     static native long indexUpdate(long indexer, java.nio.ByteBuffer block, long deviceAddr, long nbytes, boolean isFinal);   // -> consumed
+//     static native java.nio.ByteBuffer indexResult(long indexer);                                // the _name.tfrindex bytes
+//     static native long[] indexSeek(long indexer, java.nio.ByteBuffer bytes, long nbytes, long baseEntry, long baseOffset, long target);
+//     static native void indexerDestroy(long indexer);
 //   }
 #ifdef TFR_BUILD_JNI
 #include <jni.h>
@@ -59,7 +64,7 @@
 static void throw_for(JNIEnv* env, int32_t code, int64_t row) {
   const char* cls = "java/lang/RuntimeException";
   switch (code) {
-    case TFR_E_CRC_LENGTH: case TFR_E_CRC_DATA: case TFR_E_TRUNCATED: case TFR_E_RECORD_TOO_LARGE: cls = "java/io/IOException"; break;
+    case TFR_E_CRC_LENGTH: case TFR_E_CRC_DATA: case TFR_E_TRUNCATED: case TFR_E_RECORD_TOO_LARGE: case TFR_E_INDEX_MISMATCH: cls = "java/io/IOException"; break;
     case TFR_E_MALFORMED_PROTO: cls = "com/google/protobuf/InvalidProtocolBufferException"; break;
     case TFR_E_KIND_MISMATCH: case TFR_E_BAD_RECORD_TYPE: cls = "java/lang/IllegalArgumentException"; break;
     case TFR_E_EMPTY_SCALAR: cls = "java/util/NoSuchElementException"; break;
@@ -483,4 +488,37 @@ extern "C" JNIEXPORT jobjectArray JNICALL Java_com_linkedin_spark_datasources_tf
   return out;
 }
 extern "C" JNIEXPORT void JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_inferDestroy(JNIEnv*, jclass, jlong infer) { if (infer) tfr_infer_destroy((tfr_infer*)infer); }
+// the record index (recordIndex=true): the writer's close() and DefaultSource.buildIndex, and a split's seek (INTEGRATION.md)
+extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_indexerCreate(JNIEnv* env, jclass, jint device, jlong stride) {
+  tfr_indexer* h = nullptr;
+  int32_t rc = tfr_indexer_create(device, (uint64_t)stride, &h);
+  if (rc) { throw_for(env, rc, -1); return 0; }
+  return (jlong)h;
+}
+// block: a direct ByteBuffer (host bytes), or with onDevice the device address of a drained encode (tfr_encoded_result(to_host = 0))
+extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_indexUpdate(JNIEnv* env, jclass, jlong idx, jobject block, jlong deviceAddr,
+                                                                                                 jlong nbytes, jboolean isFinal) {
+  size_t used = 0;
+  const void* p = block ? env->GetDirectBufferAddress(block) : (const void*)deviceAddr;
+  int32_t rc = tfr_index_update((tfr_indexer*)idx, p, (size_t)nbytes, block ? 0 : 1, isFinal ? 1 : 0, &used);
+  if (rc) { throw_for(env, rc, -1); return 0; }
+  return (jlong)used;
+}
+extern "C" JNIEXPORT jobject JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_indexResult(JNIEnv* env, jclass, jlong idx) {
+  const void* p = nullptr; size_t n = 0;
+  int32_t rc = tfr_index_result((tfr_indexer*)idx, &p, &n);
+  if (rc) { throw_for(env, rc, -1); return nullptr; }
+  return env->NewDirectByteBuffer(const_cast<void*>(p), (jlong)n);     // owned by the indexer until indexerDestroy
+}
+// -> {entry, offset} of the first frame at or after target; bytes: the file from the checkpoint (base_entry, base_offset) on
+extern "C" JNIEXPORT jlongArray JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_indexSeek(JNIEnv* env, jclass, jlong idx, jobject bytes, jlong nbytes,
+                                                                                                      jlong baseEntry, jlong baseOffset, jlong target) {
+  int64_t e = 0, o = 0;
+  int32_t rc = tfr_index_seek((tfr_indexer*)idx, nbytes ? env->GetDirectBufferAddress(bytes) : nullptr, (size_t)nbytes, 0, baseEntry, baseOffset, target, &e, &o);
+  if (rc) { throw_for(env, rc, -1); return nullptr; }
+  jlong v[2] = {(jlong)e, (jlong)o};
+  jlongArray a = env->NewLongArray(2); env->SetLongArrayRegion(a, 0, 2, v);
+  return a;
+}
+extern "C" JNIEXPORT void JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_indexerDestroy(JNIEnv*, jclass, jlong idx) { if (idx) tfr_indexer_destroy((tfr_indexer*)idx); }
 #endif  // TFR_BUILD_JNI
