@@ -146,6 +146,39 @@ enum {
 #define TFR_SPARSE_VALUES_SUFFIX  "_values"
 #define TFR_SPARSE_SIZE_SUFFIX    "_size"
 
+/* RAGGED: the DataSource option nestedArrayFormat=ragged (`featureList`, the default, is today's behaviour; any other value is
+ * IllegalArgumentException before any work) is tfr_schema_create_ex with TFR_S_RAGGED.  In an Example schema a field
+ * x: ArrayType(ArrayType(T)) (depth 2, T any element type valid at depth 2) is stored as the two plain features
+ * tf.io.RaggedFeature(dtype, value_key = x_values, partitions = [RaggedFeature.RowLengths(x_row_lengths)]) reads:
+ *     <name>TFR_RAGGED_VALUES_SUFFIX       depth-1 list of T   the inner lists' elements, flattened in order
+ *     <name>TFR_RAGGED_ROW_LENGTHS_SUFFIX  Int64List           the inner lists' lengths
+ *   - Lowering : the values part takes x's place and nullability; the lengths part is nullable and appended after every caller
+ *              field and every sparse-vector part, in field order.  Encoded entries follow the lowered order.  To the caller x is
+ *              ONE column, laid out like a SequenceExample FeatureList column of T (depth 2, n_levels 2, or 3 for String /
+ *              Binary): tfr_schema_num_fields, tfr_batch_num_columns and the columns tfr_encode takes do not count the lengths
+ *              parts.  Feature keys that collide (ragged `x` next to a field `x_values`) are TFR_E_INVALID_ARG naming both.  A
+ *              record feature named `x` is not looked up; it is validated like any feature outside the schema.
+ *   - Schema : TFR_S_RAGGED with TFR_RT_SEQUENCE_EXAMPLE is TFR_E_INVALID_ARG (its 2-D columns are FeatureLists); a ByteArray
+ *              schema ignores the flag.  Schema inference never produces it (a ragged file infers as its two plain fields).
+ *   - Read   : both parts read by every rule of their lowered types (kinds, FAILFAST / DROPMALFORMED / PERMISSIVE, TFR_F_RESYNC,
+ *              generated fields).  Then per record: both absent -> x is null (TFR_E_NULL_IN_NONNULL when x is non-nullable,
+ *              through the values part); exactly one present -> TFR_E_BAD_NESTING at x's field index; both present -> every
+ *              length >= 0 and their sum equal to the number of values, else TFR_E_BAD_NESTING at x.  Within a record the
+ *              caller fields' errors come first (x's values part included), then the sparse-vector parts', then the lengths
+ *              parts' own errors (reported at x), and the consistency check last.
+ *   - Write  : a null x omits both features (TFR_E_NULL_IN_NONNULL when non-nullable); otherwise the flattened elements, each
+ *              through the element type's existing conversion and null-element rule, and the inner sizes.  [] writes two empty
+ *              lists; [[]] an empty values list and the lengths [0].  A null inner array (UnsafeRow input) is
+ *              TFR_E_NULL_IN_NONNULL at its row.  tfr_encode, tfr_encode_rows and tfr_encode_rows_submit alike; a tfr_encode
+ *              column whose offsets are not a depth-2 column (decreasing, negative, or past its n_offsets[1] - 1 inner
+ *              lists) is TFR_E_INVALID_ARG at the first such row.
+ *   - Paths  : every decode path takes ragged fields (tile, large-record, general, pipelined submit).  The tile and large-record
+ *              kernels do not check the parts; a batch whose parts disagree goes to the general path, which reports it.
+ * These rules restate TensorFlow's tf.io.RaggedFeature documentation and are NOT checked against TensorFlow or a JVM.          */
+#define TFR_RAGGED_VALUES_SUFFIX      "_values"
+#define TFR_RAGGED_ROW_LENGTHS_SUFFIX "_row_lengths"
+#define TFR_S_RAGGED 0x1u
+
 /* record types: the `recordType` DataSource option (M/TFRecordFileReader.scala:22,69-80) */
 enum { TFR_RT_EXAMPLE = 0, TFR_RT_SEQUENCE_EXAMPLE = 1, TFR_RT_BYTE_ARRAY = 2 };
 
@@ -177,8 +210,12 @@ const char* tfr_last_error(void);
  * `fields` are ignored.                                                                                              */
 int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, int32_t record_type,
                           tfr_schema** out);
+/* tfr_schema_create with schema flags: TFR_S_RAGGED (RAGGED above); any other bit is TFR_E_INVALID_ARG.  tfr_schema_create is
+ * this call with flags 0.                                                                                              */
+int32_t tfr_schema_create_ex(const tfr_field* fields, int32_t n_fields, int32_t record_type, uint32_t schema_flags,
+                             tfr_schema** out);
 void    tfr_schema_destroy(tfr_schema*);
-int32_t tfr_schema_num_fields(const tfr_schema*);   /* lowered: n_fields + 2 per sparse vector (SPARSE VECTORS) */
+int32_t tfr_schema_num_fields(const tfr_schema*);   /* lowered: n_fields + 2 per sparse vector (SPARSE VECTORS); ragged fields add none */
 
 /* ---- decode: replaces the body of the buildReader closure ---------------------------- */
 /* flags */

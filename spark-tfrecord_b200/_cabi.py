@@ -69,6 +69,12 @@ _LEAF_DTYPE = {TFR_T_INT32: np.int32, TFR_T_INT64: np.int64, TFR_T_FLOAT32: np.f
                TFR_T_BINARY: np.uint8, TFR_T_NULL: np.uint8}
 
 
+# RAGGED (include/tfrgpu.h): the schema flag of nestedArrayFormat=ragged and the two parts' feature-key suffixes
+TFR_S_RAGGED = 0x1
+TFR_RAGGED_VALUES_SUFFIX = "_values"
+TFR_RAGGED_ROW_LENGTHS_SUFFIX = "_row_lengths"
+
+
 def make_fields(schema: StructType, vector_format: str = "dense"):
     """StructType -> (ctypes array of tfr_field, keepalive list); VectorUDT fields by vector_format (lower_type)."""
     n = len(schema)

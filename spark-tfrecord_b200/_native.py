@@ -11,7 +11,7 @@ from typing import List, Optional
 import numpy as np
 
 from . import _cabi as A
-from ._cabi import HostColumn, column_from_ctypes, make_fields, tfr_batch_info, tfr_column, tfr_field
+from ._cabi import TFR_S_RAGGED, HostColumn, column_from_ctypes, make_fields, tfr_batch_info, tfr_column, tfr_field
 from .sqltypes import StructType
 
 _DIR = os.path.dirname(os.path.abspath(__file__))
@@ -20,7 +20,7 @@ _LIB = None
 
 # every symbol include/tfrgpu.h declares
 EXPORTS = [
-    "tfr_abi_version", "tfr_status_string", "tfr_last_error", "tfr_schema_create", "tfr_schema_destroy",
+    "tfr_abi_version", "tfr_status_string", "tfr_last_error", "tfr_schema_create", "tfr_schema_create_ex", "tfr_schema_destroy",
     "tfr_schema_num_fields", "tfr_decoder_create", "tfr_decoder_create_permissive", "tfr_decoder_destroy", "tfr_decoder_staging", "tfr_decoder_staging_slot",
     "tfr_decoder_num_staging_slots", "tfr_decode", "tfr_decode_submit", "tfr_decode_at", "tfr_decode_submit_at", "tfr_batch_extent",
     "tfr_decoder_stream", "tfr_decoder_set_profiling", "tfr_decoder_get_profile", "tfr_decoder_get_stats", "tfr_batch_wait", "tfr_batch_status", "tfr_batch_consumed", "tfr_batch_dropped", "tfr_batch_dropped_spans", "tfr_batch_num_columns", "tfr_batch_columns",
@@ -104,6 +104,7 @@ def lib():
         "tfr_status_string": (C.c_char_p, [i32]),
         "tfr_last_error": (C.c_char_p, []),
         "tfr_schema_create": (i32, [P(tfr_field), i32, i32, P(vp)]),
+        "tfr_schema_create_ex": (i32, [P(tfr_field), i32, i32, C.c_uint32, P(vp)]),
         "tfr_schema_destroy": (None, [vp]),
         "tfr_schema_num_fields": (i32, [vp]),
         "tfr_decoder_create": (i32, [vp, i32, u32, P(vp)]),
@@ -179,15 +180,17 @@ def _check(rc: int):
 
 
 class Schema:
-    def __init__(self, schema: StructType, record_type: int = 0, vector_format: str = "dense"):
+    def __init__(self, schema: StructType, record_type: int = 0, vector_format: str = "dense", ragged: bool = False):
         """`vector_format`: the `vectorFormat` option, how VectorUDT fields are stored (include/tfrgpu.h, VECTORS and SPARSE
-        VECTORS); "sparse" lowers each to three fields (sqltypes.lowered_schema), and the columns follow the lowered schema"""
+        VECTORS); "sparse" lowers each to three fields (sqltypes.lowered_schema), and the columns follow the lowered schema.
+        `ragged`: the option nestedArrayFormat=ragged (TFR_S_RAGGED, include/tfrgpu.h RAGGED); a nested array stays one
+        column."""
         self.struct = schema
         self.record_type = record_type
         self.vector_format = vector_format
         fields, self._keep = make_fields(schema, vector_format)
         h = C.c_void_p()
-        _check(lib().tfr_schema_create(fields, len(schema), record_type, C.byref(h)))
+        _check(lib().tfr_schema_create_ex(fields, len(schema), record_type, TFR_S_RAGGED if ragged else 0, C.byref(h)))
         self.h = h
 
     def close(self):
@@ -357,10 +360,10 @@ class Batch:
 
 class Decoder:
     def __init__(self, schema: StructType, record_type: int = 0, device: int = 0, flags: int = A.TFR_F_DEFAULT,
-                 corrupt_field: Optional[int] = None, vector_format: str = "dense"):
+                 corrupt_field: Optional[int] = None, vector_format: str = "dense", ragged: bool = False):
         """`corrupt_field`: with TFR_F_PERMISSIVE in `flags`, the index of the schema field that receives a failing record's
         payload (a nullable BinaryType column; tfr_decoder_create_permissive).  `vector_format`: as Schema's."""
-        self.schema = Schema(schema, record_type, vector_format)
+        self.schema = Schema(schema, record_type, vector_format, ragged)
         self.ncols = lib().tfr_schema_num_fields(self.schema.h)     # ByteArray: byteArray, then the generated fields
         h = C.c_void_p()
         if corrupt_field is None:
@@ -445,8 +448,9 @@ class Decoder:
 
 
 class Encoder:
-    def __init__(self, schema: StructType, record_type: int = 0, device: int = 0, flags: int = 0, vector_format: str = "dense"):
-        self.schema = Schema(schema, record_type, vector_format)
+    def __init__(self, schema: StructType, record_type: int = 0, device: int = 0, flags: int = 0, vector_format: str = "dense",
+                 ragged: bool = False):
+        self.schema = Schema(schema, record_type, vector_format, ragged)
         self.ncols = 1 if record_type == 2 else lib().tfr_schema_num_fields(self.schema.h)   # (a sparse vector adds two)
         h = C.c_void_p()
         _check(lib().tfr_encoder_create(self.schema.h, device, flags, C.byref(h)))

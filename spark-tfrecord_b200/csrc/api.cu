@@ -29,6 +29,7 @@
 #include "large.cuh"
 #include "permissive.cuh"
 #include "position.cuh"
+#include "ragged.cuh"
 #include "resync.cuh"
 #include "rows.cuh"
 #include "scan.cuh"
@@ -211,6 +212,15 @@ struct tfr_schema {
   bool has_vector() const { return std::find(vec.begin(), vec.end(), (uint8_t)VK_DENSE) != vec.end(); }
   // the caller's field of lowered field f: a sparse vector's part reports its vector
   int32_t owner(int32_t f) const { return f >= n_user && f < (int32_t)part.size() ? part[f] : f; }
+  // Ragged fields (include/tfrgpu.h, RAGGED): a ragged x is its values part here (depth 1) and rag_len[x] is its lengths part,
+  // one of the last n_rag fields (part[] maps it back to x).  The caller sees the first n_cols() fields as columns, x as the
+  // depth-2 column ragged.cuh assembles; the lengths parts are internal.
+  std::vector<int32_t> rag_len;
+  int32_t n_rag = 0;
+  bool ragged(int32_t f) const { return f >= 0 && f < (int32_t)rag_len.size() && rag_len[f] >= 0; }
+  int32_t n_cols() const { return (int32_t)fields.size() - n_rag; }
+  // the same fields without the ragged lowering (x at depth 2), which the UnsafeRow encoders take rows apart by
+  std::shared_ptr<tfr_schema> plain;
 };
 
 static uint32_t fnv1a(const uint8_t* p, uint32_t n) { uint32_t h = 2166136261u; for (uint32_t i = 0; i < n; ++i) h = (h ^ p[i]) * 16777619u; return h; }
@@ -238,9 +248,16 @@ static bool add_generated(tfr_schema& s, const tfr_field& f, const std::string& 
 static void schema_rehash(tfr_schema& s, int32_t skip);
 
 extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, int32_t record_type, tfr_schema** out) {
+  return tfr_schema_create_ex(fields, n_fields, record_type, 0, out);
+}
+extern "C" int32_t tfr_schema_create_ex(const tfr_field* fields, int32_t n_fields, int32_t record_type, uint32_t schema_flags,
+                                        tfr_schema** out) {
   if (!out || n_fields < 0 || (n_fields > 0 && !fields)) return fail(TFR_E_INVALID_ARG, "null argument");
+  if (schema_flags & ~TFR_S_RAGGED) return fail(TFR_E_INVALID_ARG, "unknown schema flags");
   if (record_type < TFR_RT_EXAMPLE || record_type > TFR_RT_BYTE_ARRAY)
     return fail(TFR_E_BAD_RECORD_TYPE, "Unsupported recordType: recordType can be ByteArray, Example or SequenceExample");
+  if ((schema_flags & TFR_S_RAGGED) && record_type == TFR_RT_SEQUENCE_EXAMPLE)
+    return fail(TFR_E_INVALID_ARG, "nestedArrayFormat=ragged is for Example records: SequenceExample stores nested arrays as FeatureLists");
   if (n_fields > 4096) return fail(TFR_E_INVALID_ARG, "more than 4096 fields");
   auto s = std::make_unique<tfr_schema>();
   s->record_type = record_type;
@@ -267,6 +284,7 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
     }
     s->vec.assign(s->fields.size(), VK_NONE);
     s->part.assign(s->fields.size(), -1);
+    s->rag_len.assign(s->fields.size(), -1);
     s->n_user = (int32_t)s->fields.size();
     *out = s.release();
     return TFR_OK;
@@ -292,16 +310,17 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
     s->fields.push_back(d);
     s->vec.push_back(vk);
     s->part.push_back(part);
+    s->rag_len.push_back(-1);
   };
   std::vector<std::string> user(n_fields);              // the caller's names
-  std::vector<int32_t> sparse;                          // the sparse vectors, in field order
+  std::vector<int32_t> sparse, ragged;                  // the sparse vectors and the ragged fields, in field order
   for (int32_t i = 0; i < n_fields; ++i) {
     const tfr_field& f = fields[i];
     if (f.name_len < 0 || (f.name_len > 0 && !f.name)) return fail(TFR_E_INVALID_ARG, "bad field name");
     std::string nm(f.name ? f.name : "", (size_t)f.name_len);
     user[i] = nm;
     int32_t rc = TFR_OK;
-    if (add_generated(*s, f, nm, &rc)) { if (rc) return rc; s->vec.push_back(VK_NONE); s->part.push_back(-1); continue; }
+    if (add_generated(*s, f, nm, &rc)) { if (rc) return rc; s->vec.push_back(VK_NONE); s->part.push_back(-1); s->rag_len.push_back(-1); continue; }
     // a VectorUDT field is an ArrayType(DoubleType) field to every kernel but the UnsafeRow ones (VECTORS); a sparse one is
     // its values field here, and its indices and size fields are appended below (SPARSE VECTORS)
     const bool vector = f.elem_type == TFR_T_VECTOR, sp = f.elem_type == TFR_T_SPARSE_VECTOR;
@@ -312,7 +331,11 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
     bool ok_type = et >= TFR_T_NULL && et <= TFR_T_BINARY && depth >= 0 && depth <= 2 && !(et == TFR_T_NULL && depth > 0);
     if (!ok_type) return fail(TFR_E_UNSUPPORTED_TYPE, "field '" + nm + "': data type is not supported");
     if (sp) sparse.push_back(i);
-    add(sp ? nm + TFR_SPARSE_VALUES_SUFFIX : nm, et, depth, f.nullable != 0, vector ? VK_DENSE : sp ? VK_SPARSE : VK_NONE, -1);
+    // a ragged field is its values part here (depth 1), and its lengths part is appended below (RAGGED)
+    const bool rg = (schema_flags & TFR_S_RAGGED) && record_type == TFR_RT_EXAMPLE && depth == 2;
+    if (rg) ragged.push_back(i);
+    add(sp ? nm + TFR_SPARSE_VALUES_SUFFIX : rg ? nm + TFR_RAGGED_VALUES_SUFFIX : nm, et, rg ? 1 : depth, f.nullable != 0,
+        vector ? VK_DENSE : sp ? VK_SPARSE : VK_NONE, -1);
   }
   s->n_user = n_fields;
   for (int32_t v : sparse) {
@@ -320,11 +343,21 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
     add(user[v] + TFR_SPARSE_INDICES_SUFFIX, TFR_T_INT32, 1, true, VK_INDICES, v);
     add(user[v] + TFR_SPARSE_SIZE_SUFFIX, TFR_T_INT32, 0, true, VK_SIZE, v);
   }
+  for (int32_t x : ragged) {
+    s->rag_len[x] = (int32_t)s->fields.size();
+    add(user[x] + TFR_RAGGED_ROW_LENGTHS_SUFFIX, TFR_T_INT64, 1, true, VK_NONE, x);
+  }
+  s->n_rag = (int32_t)ragged.size();
+  if (s->n_rag) {
+    tfr_schema* p = nullptr;
+    TRY(tfr_schema_create_ex(fields, n_fields, record_type, 0, &p));
+    s->plain.reset(p);
+  }
   // Spark refuses duplicate column names for file sources before the reader is built
   // (SchemaUtils.checkColumnNameDuplication), so they never reach TFRecordDeserializer
   if (std::unordered_set<std::string>(user.begin(), user.end()).size() != user.size())
     return fail(TFR_E_INVALID_ARG, "Found duplicate column(s) in the data schema");
-  // and two fields may not share a feature key, which only a sparse vector's keys can do past the check above
+  // and two fields may not share a feature key, which only a sparse vector's or a ragged field's keys can do past the check above
   const int32_t nl = (int32_t)s->fields.size();
   auto key = [&](int32_t f) { const DevField& d = s->fields[f]; return std::string((const char*)&s->names[d.name_off], d.name_len); };
   size_t hsz = 2; while (hsz < 2 * (size_t)nl + 2) hsz <<= 1;
@@ -358,13 +391,14 @@ static void schema_rehash(tfr_schema& s, int32_t skip) {
   }
 }
 extern "C" void tfr_schema_destroy(tfr_schema* s) { delete s; }
-extern "C" int32_t tfr_schema_num_fields(const tfr_schema* s) { return s ? (int32_t)s->fields.size() : 0; }
+extern "C" int32_t tfr_schema_num_fields(const tfr_schema* s) { return s ? s->n_cols() : 0; }
 
 // device copy of a schema.  The copies run on the handle's stream `st` and are waited for before returning: the handle's
 // kernels run on non-blocking streams, which nothing orders after the legacy default stream, and `tp` is a local.
 struct DevSchemaBuf {
   DevBuf fields, names, ht, var_field, templates;
   DevBuf vec, part;                                       // tfr_schema::vec and ::part, for the UnsafeRow kernels of the encoder
+  DevBuf rag; int32_t n_rag = 0;                          // pairs (ragged field, its lengths part), for decode_pass1_kernel<true>
   DevBuf tile_consts; uint32_t tile_consts_bytes = 0;     // tile.cuh: per-schema constants in the shared-memory layout
   DevSchema view{};
   const int32_t* d_var_field() const { return (const int32_t*)var_field.p; }
@@ -386,6 +420,11 @@ struct DevSchemaBuf {
     if (!s.names.empty()) CUDA_TRY(cudaMemcpyAsync(names.p, s.names.data(), s.names.size(), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(ht.p, s.ht.data(), s.ht.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     if (!s.var_field.empty()) CUDA_TRY(cudaMemcpyAsync(var_field.p, s.var_field.data(), s.var_field.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    std::vector<int32_t> pairs;
+    for (int32_t f = 0; f < s.n_cols(); ++f) if (s.ragged(f)) { pairs.push_back(f); pairs.push_back(s.rag_len[f]); }
+    n_rag = (int32_t)pairs.size() / 2;
+    CUDA_TRY(rag.alloc(std::max<size_t>(2, pairs.size()) * sizeof(int32_t)));
+    if (!pairs.empty()) CUDA_TRY(cudaMemcpyAsync(rag.p, pairs.data(), pairs.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     {
       // canonical entry prefix of every field: 0A ? 0A klen key 12 ? kindtag ?   (? = length bytes, masked out)
       std::vector<FieldTemplate> tp(std::max<size_t>(1, nf));
@@ -536,6 +575,7 @@ extern "C" int32_t tfr_batch_export_arrow_host(tfr_batch* b, int32_t column, voi
   const tfr_column& c = b->host_copy.cols[column];
   const tfr_schema& S = b->dec->schema;
   std::string nm((const char*)&S.names[S.fields[column].name_off], S.fields[column].name_len);
+  if (S.ragged(column)) nm.resize(nm.size() - strlen(TFR_RAGGED_VALUES_SUFFIX));     // x, not its values part's key
   build_schema((ArrowSchema*)arrow_schema, nm.c_str(), c.elem_type, c.depth);
   build_array((ArrowArray*)arrow_array, c, 0, c.n_rows, b);
   return TFR_OK;
@@ -547,6 +587,7 @@ extern "C" int32_t tfr_batch_export_arrow_device(tfr_batch* b, int32_t column, v
   const tfr_column& c = b->out.cols[column];
   const tfr_schema& S = b->dec->schema;
   std::string nm((const char*)&S.names[S.fields[column].name_off], S.fields[column].name_len);
+  if (S.ragged(column)) nm.resize(nm.size() - strlen(TFR_RAGGED_VALUES_SUFFIX));     // x, not its values part's key
   build_schema((ArrowSchema*)arrow_schema, nm.c_str(), c.elem_type, c.depth);
   auto* da = (ArrowDeviceArray*)arrow_device_array;
   memset(da, 0, sizeof *da);

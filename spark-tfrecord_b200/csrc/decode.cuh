@@ -46,6 +46,9 @@ struct DecodeArgs {
   const int32_t* var_field;   // [n_var] schema field of each var slot
   uint32_t flist_warp;        // 1: canonical FeatureList cells with fixed-width elements are emitted by decode_pass2_flist_kernel
   uint32_t canon_lean;        // 1: scalar string/binary cells and canonical 1-D list cells are emitted by decode_pass2_canon_kernel
+  // pass 1 of a schema with ragged fields (decode_pass1_kernel<true>): [n_rag] pairs (x, its lengths part)
+  const int32_t* rag;
+  uint32_t n_rag;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -361,6 +364,54 @@ __device__ __forceinline__ bool walk_map_body(const DecodeArgs& A, uint32_t row,
   }
 }
 
+// a ragged field's consistency check (ragged.cuh): the sum of the lengths part's values in row `row` (the final run of the winning
+// entry, by Feature's merge rules: a list of another kind discards what came before), ~0 when one is negative or above INT32_MAX.
+// `src`: the packed varints (cflag CF_CANON, `count` of them) or the map entry's length prefix (CF_GENERAL).
+__device__ __forceinline__ uint64_t ragged_lengths_sum(const uint8_t* data, uint32_t nbytes, uint32_t src, bool canon, uint32_t count) {
+  uint64_t sum = 0;
+  bool bad = false;
+  auto add = [&](uint64_t v) { if (v > 0x7fffffffull) bad = true; else sum += v; };
+  if (canon) {
+    Cur pk{data + src, data + nbytes};
+    for (uint32_t i = 0; i < count; ++i) { uint64_t v; if (!rd_varint64(pk, v)) return ~0ull; add(v); }
+    return bad ? ~0ull : sum;
+  }
+  Cur c{data + src, data + nbytes};
+  uint32_t l;
+  if (!rd_len(c, l)) return ~0ull;
+  Cur e{c.p, c.p + l};
+  for (;;) {                                                   // MapEntry: value = 2 (repeated occurrences merge)
+    uint32_t tag;
+    if (!rd_tag(e, tag)) return ~0ull;
+    if (tag == 0) break;
+    if (tag != 0x12) { if (!skip_field(e, tag)) return ~0ull; continue; }
+    if (!rd_len(e, l)) return ~0ull;
+    Cur f{e.p, e.p + l};
+    e.p += l;
+    for (;;) {                                                 // Feature: bytes_list = 1, float_list = 2, int64_list = 3
+      if (!rd_tag(f, tag)) return ~0ull;
+      if (tag == 0) break;
+      if (tag != 0x0A && tag != 0x12 && tag != 0x1A) { if (!skip_field(f, tag)) return ~0ull; continue; }
+      if (!rd_len(f, l)) return ~0ull;
+      Cur b{f.p, f.p + l};
+      f.p += l;
+      if (tag != 0x1A) { sum = 0; bad = false; continue; }    // the oneof switches: the int64 values before it are discarded
+      for (;;) {                                               // Int64List: value = 1, packed or not
+        if (!rd_tag(b, tag)) return ~0ull;
+        if (tag == 0) break;
+        if (tag == 0x08) { uint64_t v; if (!rd_varint64(b, v)) return ~0ull; add(v); }
+        else if (tag == 0x0A) {
+          if (!rd_len(b, l)) return ~0ull;
+          Cur pk{b.p, b.p + l};
+          while (pk.p < pk.end) { uint64_t v; if (!rd_varint64(pk, v)) return ~0ull; add(v); }
+          b.p += l;
+        } else if (!skip_field(b, tag)) return ~0ull;
+      }
+    }
+  }
+  return bad ? ~0ull : sum;
+}
+
 // a row that fails before the per-field epilogue (bad CRC, malformed proto): zero counts, null validity
 __device__ __forceinline__ void null_fill_row(const DecodeArgs& A, uint32_t row) {
   const uint32_t lane = threadIdx.x & 31;
@@ -368,6 +419,8 @@ __device__ __forceinline__ void null_fill_row(const DecodeArgs& A, uint32_t row)
   for (uint32_t c = lane; c < (uint32_t)A.sch.n_cnt; c += 32) A.cnt[(size_t)c * A.n + row] = 0;
 }
 
+// RG: the schema has ragged fields, whose parts must agree (RAGGED, include/tfrgpu.h); without them the kernel is unchanged
+template <bool RG>
 __global__ void __launch_bounds__(256) decode_pass1_kernel(DecodeArgs A) {
   extern __shared__ uint32_t smem[];
   uint32_t* stab = smem;
@@ -452,6 +505,28 @@ __global__ void __launch_bounds__(256) decode_pass1_kernel(DecodeArgs A) {
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) worst = min(worst, __shfl_xor_sync(FULLMASK, worst, o));
+    if constexpr (RG) {
+      // last in a record's precedence: a ragged field whose parts disagree (one absent, a negative length, a wrong sum) is
+      // TFR_E_BAD_NESTING at x; the first such x in field order
+      if (worst == 0xffffffffu) {
+        uint32_t bad = 0xffffffffu;
+        for (uint32_t j = lane; j < A.n_rag; j += 32) {
+          const int x = A.rag[2 * j], L = A.rag[2 * j + 1];
+          const bool px = (fstate[x] & 0x3f) == 1, pl = (fstate[L] & 0x3f) == 1;
+          bool mis = px != pl;
+          if (px && pl) {
+            const DevField& fl = A.sch.fields[L];
+            const size_t vs = (size_t)fl.var_slot * A.n + row;
+            const uint64_t sum = ragged_lengths_sum(A.data, A.nbytes, A.src[vs], A.cflag[vs] == CF_CANON, A.cnt[(size_t)fl.cnt_slot * A.n + row]);
+            mis = sum != (uint64_t)A.cnt[(size_t)A.sch.fields[x].cnt_slot * A.n + row];
+          }
+          if (mis) bad = min(bad, (uint32_t)x);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) bad = min(bad, __shfl_xor_sync(FULLMASK, bad, o));
+        if (bad != 0xffffffffu) worst = (bad << 8) | (uint32_t)(-TFR_E_BAD_NESTING);
+      }
+    }
     if (lane == 0) A.status[row] = worst == 0xffffffffu ? 0u : ((worst & 0xff) | (((worst >> 8) + 1) << 8));
   }
 }

@@ -70,6 +70,19 @@ def _vector_format(options: Optional[Dict[str, str]]) -> str:
         raise _native.IllegalArgumentException(-1, str(e)) from None
 
 
+def _nested_array_format(options: Optional[Dict[str, str]]) -> bool:
+    """the `nestedArrayFormat` option: True for "ragged", where an Example's ArrayType(ArrayType(T)) field x is the two plain
+    features x_values and x_row_lengths of tf.io.RaggedFeature (include/tfrgpu.h, RAGGED); "featureList" (the default) is the
+    reference's behaviour.  Anything else, and ragged with recordType=SequenceExample, is refused before any work."""
+    nf = (options or {}).get("nestedArrayFormat", "featureList")
+    if nf not in ("featureList", "ragged"):
+        raise _native.IllegalArgumentException(-1, f"nestedArrayFormat {nf}: the option takes featureList or ragged")
+    if nf == "ragged" and (options or {}).get("recordType", "Example") == "SequenceExample":
+        raise _native.IllegalArgumentException(-1, "nestedArrayFormat=ragged is for Example records: SequenceExample stores "
+                                                   "nested arrays as FeatureLists")
+    return nf == "ragged"
+
+
 def _corrupt_column_name(options: Optional[Dict[str, str]]) -> str:
     """the option columnNameOfCorruptRecord, named and defaulted as Spark's JSON and CSV sources have it"""
     return (options or {}).get("columnNameOfCorruptRecord", "_corrupt_record")
@@ -470,12 +483,13 @@ class TFRecordFileReader:
         stream for a compressed file), filled on the GPU.  ByteArray rows are byteArray, then those fields."""
         rt = _record_type(options)
         vf = _vector_format(options)
+        ragged = _nested_array_format(options)
         flags, corrupt = _read_mode(options, schema if dataSchema is None else dataSchema, schema)
         block = block_bytes or TFRecordFileReader.BLOCK_BYTES
         # recordIndex=true: a split of a file reads exactly the frames whose header offset lies in it (RECORD INDEX)
         split = (_record_index(options) and _codec_of_path(file.toPath()) is None
                  and (file.start, file.length) != (0, os.path.getsize(file.toPath())))
-        dec = _native.Decoder(_decoder_schema(schema), rt, device, flags, corrupt_field=corrupt, vector_format=vf)
+        dec = _native.Decoder(_decoder_schema(schema), rt, device, flags, corrupt_field=corrupt, vector_format=vf, ragged=ragged)
 
         def gen():
             todo = []
@@ -583,7 +597,8 @@ class TFRecordOutputWriter:
         self.recordType = _record_type(options)                 # validated up front; the reference throws at the first write
         self.schema = byte_array_schema() if self.recordType == 2 else dataSchema
         self.vectorFormat = _vector_format(options)
-        self._enc = _native.Encoder(self.schema, self.recordType, device, vector_format=self.vectorFormat)
+        self._enc = _native.Encoder(self.schema, self.recordType, device, vector_format=self.vectorFormat,
+                                    ragged=_nested_array_format(options))
         self._rows: List[tuple] = []
         self._bytes = 0
         codec = _codec_name((options or {}).get("codec", ""))
@@ -709,6 +724,7 @@ class DefaultSource:
         columnNameOfCorruptRecord and always ends the schema with that column (nullable BinaryType), so that the schema
         reads the files back under the options it was inferred with (buildReader refuses PERMISSIVE without it)."""
         from .sharding import allreduce_schema, codes_to_struct, shard_lpt
+        _nested_array_format(options)                 # validated; a ragged file infers as its two plain fields
         mode, flags = _mode_flags(options)
         rt = _record_type(options)
         if rt == 2:
@@ -768,12 +784,14 @@ class DefaultSource:
         DROPMALFORMED, or PERMISSIVE when `dataSchema` holds the corrupt-record column, checked here, before any file is read."""
         _read_mode(options, dataSchema, requiredSchema)
         _vector_format(options)
+        _nested_array_format(options)
         _record_index(options)
         return lambda file: TFRecordFileReader.readFile(None, options, file, requiredSchema, device, dataSchema=dataSchema)
 
     def prepareWrite(self, options: Dict[str, str], dataSchema: StructType):
         codec = _codec_name((options or {}).get("codec", ""))             # :94-102: the option turns output compression on
         _vector_format(options)
+        _nested_array_format(options)
         _check_record_index(options, codec)
 
         class _Factory:

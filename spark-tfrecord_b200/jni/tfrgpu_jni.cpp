@@ -5,6 +5,8 @@
 // Java side (package com.linkedin.spark.datasources.tfrecord):
 //   final class TfrGpu {
 //     static native long schemaCreate(String[] names, int[] elemTypes, int[] depths, boolean[] nullable, int recordType);
+//     static native long schemaCreateFormat(String[] names, int[] elemTypes, int[] depths, boolean[] nullable, int recordType,
+//                                           String nestedArrayFormat);   // "featureList" (schemaCreate) or "ragged": TFR_S_RAGGED
 //     static native int udtElemType(String udtClassName);   // a UserDefinedType's TFR_T_* by class name (VectorUDT: 10), -1 none
 //     static native int udtElemTypeFormat(String udtClassName, String vectorFormat);   // the same under the vectorFormat option:
 //                                                 // VectorUDT 10 (dense) or 11 (sparse), -1 another UDT, -2 another format
@@ -76,8 +78,8 @@ static void throw_for(JNIEnv* env, int32_t code, int64_t row) {
   env->ThrowNew(env->FindClass(cls), msg.c_str());
 }
 
-extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_schemaCreate(
-    JNIEnv* env, jclass, jobjectArray names, jintArray elemTypes, jintArray depths, jbooleanArray nullable, jint recordType) {
+static jlong schema_create(JNIEnv* env, jobjectArray names, jintArray elemTypes, jintArray depths, jbooleanArray nullable,
+                           jint recordType, uint32_t schema_flags) {
   jsize n = env->GetArrayLength(names);
   std::vector<std::string> keep(n);
   std::vector<tfr_field> f(n);
@@ -91,11 +93,36 @@ extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_
     f[i] = tfr_field{keep[i].data(), (int32_t)keep[i].size(), et[i], dp[i], nl[i] ? 1 : 0};
   }
   tfr_schema* out = nullptr;
-  int32_t rc = tfr_schema_create(f.data(), n, recordType, &out);
+  int32_t rc = tfr_schema_create_ex(f.data(), n, recordType, schema_flags, &out);
   env->ReleaseIntArrayElements(elemTypes, et, JNI_ABORT); env->ReleaseIntArrayElements(depths, dp, JNI_ABORT);
   env->ReleaseBooleanArrayElements(nullable, nl, JNI_ABORT);
   if (rc) { throw_for(env, rc, -1); return 0; }
   return (jlong)out;
+}
+extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_schemaCreate(
+    JNIEnv* env, jclass, jobjectArray names, jintArray elemTypes, jintArray depths, jbooleanArray nullable, jint recordType) {
+  return schema_create(env, names, elemTypes, depths, nullable, recordType, 0);
+}
+// DefaultSource's nestedArrayFormat option (include/tfrgpu.h, RAGGED) as schema flags: "featureList" 0, "ragged" TFR_S_RAGGED;
+// -1 (IllegalArgumentException) for any other value, and for ragged with recordType=SequenceExample
+static int64_t nested_array_flags(const std::string& format, int32_t record_type) {
+  if (format == "featureList") return 0;
+  if (format == "ragged" && record_type != TFR_RT_SEQUENCE_EXAMPLE) return TFR_S_RAGGED;
+  return -1;
+}
+extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_schemaCreateFormat(
+    JNIEnv* env, jclass, jobjectArray names, jintArray elemTypes, jintArray depths, jbooleanArray nullable, jint recordType,
+    jstring nestedArrayFormat) {
+  const char* u = env->GetStringUTFChars(nestedArrayFormat, nullptr);
+  const std::string fmt = u ? u : "";
+  if (u) env->ReleaseStringUTFChars(nestedArrayFormat, u);
+  const int64_t flags = nested_array_flags(fmt, recordType);
+  if (flags < 0) {
+    env->ThrowNew(env->FindClass("java/lang/IllegalArgumentException"),
+                  ("nestedArrayFormat " + fmt + ": featureList, or ragged for Example records").c_str());
+    return 0;
+  }
+  return schema_create(env, names, elemTypes, depths, nullable, recordType, (uint32_t)flags);
 }
 // The element type of a UserDefinedType field, by the UDT's class name, so that the glue needs no compile-time dependency on
 // spark-mllib: both VectorUDTs (same sqlType) are TFR_T_VECTOR; any other UDT is -1 (unsupported, as in the reference).
