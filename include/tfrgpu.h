@@ -72,7 +72,13 @@ enum {
   TFR_T_ROW_INDEX     = 8,  /* the row's entry index in its file                                */
   TFR_T_RECORD_OFFSET = 9,  /* the file offset of the row's entry                               */
   TFR_T_VECTOR        = 10, /* Spark ML's VectorUDT, read and written as a FloatList (VECTORS below) */
-  TFR_T_SPARSE_VECTOR = 11  /* Spark ML's VectorUDT, read and written as TF sparse features (SPARSE VECTORS below) */
+  TFR_T_SPARSE_VECTOR = 11, /* Spark ML's VectorUDT, read and written as TF sparse features (SPARSE VECTORS below) */
+  /* Stored as an Int64List (INT64 TYPES below); only with the schema flag TFR_S_INT64_TYPES */
+  TFR_T_BOOL      = 12, /* BooleanType                                                        */
+  TFR_T_INT8      = 13, /* ByteType                                                           */
+  TFR_T_INT16     = 14, /* ShortType                                                          */
+  TFR_T_DATE      = 15, /* DateType: days since 1970-01-01                                    */
+  TFR_T_TIMESTAMP = 16  /* TimestampType: microseconds since the epoch, UTC                   */
 };
 /* VECTORS: TFR_T_VECTOR is org.apache.spark.ml.linalg.VectorUDT (and org.apache.spark.mllib.linalg.VectorUDT, which has the
  * same sqlType: struct<type: tinyint not null, size: int, indices: array<int not null>, values: array<double not null>>).
@@ -179,6 +185,38 @@ enum {
 #define TFR_RAGGED_ROW_LENGTHS_SUFFIX "_row_lengths"
 #define TFR_S_RAGGED 0x1u
 
+/* INT64 TYPES: the DataSource option extendedTypes=true (`false`, the default, refuses these types as before; any other value is
+ * IllegalArgumentException before any work) is tfr_schema_create_ex with TFR_S_INT64_TYPES, which may be combined with
+ * TFR_S_RAGGED.  Without the flag the five ids below are TFR_E_UNSUPPORTED_TYPE naming the field; a ByteArray schema ignores it.
+ *     type               tfr_column value_width   written as the Int64           read from Int64 v          Arrow format
+ *     TFR_T_BOOL         1 (one byte, 0 or 1)     0 or 1 (a nonzero byte is 1)   v != 0, over all 64 bits   b (bit-packed)
+ *     TFR_T_INT8         1                        sign-extended                  the low 8 bits             c
+ *     TFR_T_INT16        2                        sign-extended                  the low 16 bits            s
+ *     TFR_T_DATE         4                        days, sign-extended            the low 32 bits            tdD
+ *     TFR_T_TIMESTAMP    8                        microseconds, UTC              v                          tsu:UTC
+ *   - Lowering : such a field IS a LongType field of the same name, depth (0, 1, 2) and nullability; every rule follows from that
+ *              one (kinds: a FloatList or BytesList is TFR_E_KIND_MISMATCH; .head of an empty list is TFR_E_EMPTY_SCALAR; nulls,
+ *              non-nullable fields, SequenceExample context and FeatureLists, ragged fields, FAILFAST / DROPMALFORMED /
+ *              PERMISSIVE, TFR_F_RESYNC, generated fields, every decode path).  The file bytes are those of the LongType field
+ *              holding the widened values, so a reader without the flag, or TensorFlow, reads the file as LongType.  Schema
+ *              inference never produces these types: an Int64List infers as LongType.
+ *   - Read   : the field is parsed as LongType; then one kernel launch per batch narrows every such column's leaf values (all
+ *              but TFR_T_TIMESTAMP, whose int64 values are its own) into the batch's outputs, and writes a boolean column's
+ *              bit-packed values too.  Offsets and validity are the LongType column's.  tfr_column reports the type above and
+ *              its value_width; the leaf values are in the narrow type.  tfr_batch_export_arrow_host / _device hand out the
+ *              format above (a boolean's values buffer is the bit-packed one, bits past the length zero).
+ *   - Rows   : tfr_batch_rows (and _with_partition, _async) write what UnsafeRowWriter and UnsafeArrayData write: a scalar slot
+ *              is zeroed, then holds 1 (boolean 0/1), 1, 2, 4 or 8 bytes; an array element is 1, 1, 2, 4 or 8 bytes wide, and
+ *              the element region is rounded up to 8 bytes and zero-padded.
+ *   - Write, tfr_encode : a column of these types has to carry its value_width (above), else TFR_E_INVALID_ARG.  One widening
+ *              launch turns every such column into int64 leaf values; a nonzero boolean byte becomes 1.
+ *   - Write, tfr_encode_rows / tfr_encode_rows_submit : the rows hold the layouts of Rows above; a slot or element is read
+ *              at its width and widened as in the table (a boolean byte read from a row is != 0, a byte, short or date is
+ *              sign-extended).  Every existing row check applies to each offset and size, with the element width of the type.
+ *              A null element of an array follows LongType's rule: its slot's bits are written.
+ * The UnsafeRow layouts are restated from Spark's UnsafeRowWriter and UnsafeArrayData and are NOT checked against a JVM.      */
+#define TFR_S_INT64_TYPES 0x4u
+
 /* record types: the `recordType` DataSource option (M/TFRecordFileReader.scala:22,69-80) */
 enum { TFR_RT_EXAMPLE = 0, TFR_RT_SEQUENCE_EXAMPLE = 1, TFR_RT_BYTE_ARRAY = 2 };
 
@@ -210,7 +248,7 @@ const char* tfr_last_error(void);
  * `fields` are ignored.                                                                                              */
 int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, int32_t record_type,
                           tfr_schema** out);
-/* tfr_schema_create with schema flags: TFR_S_RAGGED (RAGGED above); any other bit is TFR_E_INVALID_ARG.  tfr_schema_create is
+/* tfr_schema_create with schema flags: TFR_S_RAGGED (RAGGED above), TFR_S_INT64_TYPES (INT64 TYPES above); any other bit is TFR_E_INVALID_ARG.  tfr_schema_create is
  * this call with flags 0.                                                                                              */
 int32_t tfr_schema_create_ex(const tfr_field* fields, int32_t n_fields, int32_t record_type, uint32_t schema_flags,
                              tfr_schema** out);

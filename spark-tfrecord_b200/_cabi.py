@@ -10,7 +10,8 @@ import numpy as np
 
 from .sqltypes import (StructType, lower_type, TFR_T_NULL, TFR_T_INT32, TFR_T_INT64, TFR_T_FLOAT32,
                        TFR_T_FLOAT64, TFR_T_DECIMAL, TFR_T_STRING, TFR_T_BINARY, TFR_T_ROW_INDEX, TFR_T_RECORD_OFFSET,
-                       TFR_T_VECTOR, TFR_T_SPARSE_VECTOR, lowered_schema, sparse_parts, sparse_vector_fields)
+                       TFR_T_VECTOR, TFR_T_SPARSE_VECTOR, lowered_schema, sparse_parts, sparse_vector_fields,
+                       TFR_T_BOOL, TFR_T_INT8, TFR_T_INT16, TFR_T_DATE, TFR_T_TIMESTAMP, INT64_TYPES, int64_leaf, int64_value)
 
 TFR_OK = 0
 TFR_E_INVALID_ARG = -1
@@ -66,24 +67,28 @@ class tfr_column(C.Structure):
 
 _LEAF_DTYPE = {TFR_T_INT32: np.int32, TFR_T_INT64: np.int64, TFR_T_FLOAT32: np.float32,
                TFR_T_FLOAT64: np.float64, TFR_T_DECIMAL: np.float64, TFR_T_STRING: np.uint8,
-               TFR_T_BINARY: np.uint8, TFR_T_NULL: np.uint8}
+               TFR_T_BINARY: np.uint8, TFR_T_NULL: np.uint8,
+               TFR_T_BOOL: np.uint8, TFR_T_INT8: np.int8, TFR_T_INT16: np.int16, TFR_T_DATE: np.int32, TFR_T_TIMESTAMP: np.int64}
 
 
 # RAGGED (include/tfrgpu.h): the schema flag of nestedArrayFormat=ragged and the two parts' feature-key suffixes
 TFR_S_RAGGED = 0x1
 TFR_RAGGED_VALUES_SUFFIX = "_values"
 TFR_RAGGED_ROW_LENGTHS_SUFFIX = "_row_lengths"
+# INT64 TYPES (include/tfrgpu.h): the schema flag of extendedTypes=true
+TFR_S_INT64_TYPES = 0x4
 
 
-def make_fields(schema: StructType, vector_format: str = "dense"):
-    """StructType -> (ctypes array of tfr_field, keepalive list); VectorUDT fields by vector_format (lower_type)."""
+def make_fields(schema: StructType, vector_format: str = "dense", extended_types: bool = False):
+    """StructType -> (ctypes array of tfr_field, keepalive list); VectorUDT fields by vector_format, BooleanType .. TimestampType
+    by extended_types (lower_type)."""
     n = len(schema)
     arr = (tfr_field * max(n, 1))()
     keep = []
     for i, f in enumerate(schema):
         nm = f.name.encode("utf-8") if isinstance(f.name, str) else bytes(f.name)
         keep.append(nm)
-        t, d = lower_type(f.dataType, vector_format)
+        t, d = lower_type(f.dataType, vector_format, extended_types)
         arr[i].name = nm
         arr[i].name_len = len(nm)
         arr[i].elem_type = t
@@ -125,6 +130,8 @@ class HostColumn:
                 b = self.values[so[i]:so[i + 1]].tobytes()
                 out.append(b.decode("utf-8") if self.elem_type == TFR_T_STRING else b)
             return out
+        if self.elem_type in INT64_TYPES:
+            return [int64_value(self.elem_type, v) for v in self.values[lo:hi].tolist()]
         return [v.item() for v in self.values[lo:hi]]
 
     def get(self, r: int):
@@ -189,8 +196,9 @@ def columns_from_rows(schema: StructType, rows: Sequence[Sequence], record_type:
     cols = []
     n = len(rows)
     for ci, f in enumerate(schema):
-        t, depth = lower_type(f.dataType)
+        t, depth = lower_type(f.dataType, extended_types=True)   # (a schema without the option refused these types already)
         vector = t == TFR_T_VECTOR and depth == 0
+        i64t = t in INT64_TYPES
         if vector:
             t, depth = TFR_T_FLOAT64, 1
         dt = _LEAF_DTYPE.get(t, np.uint8)
@@ -207,7 +215,7 @@ def columns_from_rows(schema: StructType, rows: Sequence[Sequence], record_type:
                 leafbytes.extend(b)
                 offs[nlev - 1].append(len(leafbytes))
             else:
-                leaves.append(v)
+                leaves.append(int64_leaf(t, v) if i64t else v)
 
         def leaf_count():
             return (len(offs[nlev - 1]) - 1) if varlen else len(leaves)

@@ -27,6 +27,7 @@
 #include "index.cuh"
 #include "infer.cuh"
 #include "large.cuh"
+#include "narrow.cuh"
 #include "permissive.cuh"
 #include "position.cuh"
 #include "ragged.cuh"
@@ -221,6 +222,15 @@ struct tfr_schema {
   int32_t n_cols() const { return (int32_t)fields.size() - n_rag; }
   // the same fields without the ragged lowering (x at depth 2), which the UnsafeRow encoders take rows apart by
   std::shared_ptr<tfr_schema> plain;
+  // INT64 TYPES (include/tfrgpu.h): the caller's TFR_T_BOOL .. TFR_T_TIMESTAMP of a field lowered to TFR_T_INT64, 0 otherwise.
+  // Every parse and encode kernel sees the LongType field; narrow.cuh converts its leaf values at the edges.
+  std::vector<int8_t> nar;
+  int32_t nar_type(int32_t f) const { return f >= 0 && f < (int32_t)nar.size() ? nar[f] : 0; }
+  // a column whose leaf values narrow.cuh converts (a timestamp's int64 values are its own)
+  bool narrowed(int32_t f) const { const int32_t t = nar_type(f); return t != 0 && t != TFR_T_TIMESTAMP; }
+  bool has_narrowed() const { for (int32_t f = 0; f < (int32_t)nar.size(); ++f) if (narrowed(f)) return true; return false; }
+  // a field of a 1- or 2-byte type, whose UnsafeRow slots and array elements only urows_emit_kernel<*, true> writes
+  bool has_narrow_row_field() const { for (int32_t f = 0; f < (int32_t)nar.size(); ++f) if (narrowed(f) && nar_width(nar[f]) < 4) return true; return false; }
 };
 
 static uint32_t fnv1a(const uint8_t* p, uint32_t n) { uint32_t h = 2166136261u; for (uint32_t i = 0; i < n; ++i) h = (h ^ p[i]) * 16777619u; return h; }
@@ -253,7 +263,7 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
 extern "C" int32_t tfr_schema_create_ex(const tfr_field* fields, int32_t n_fields, int32_t record_type, uint32_t schema_flags,
                                         tfr_schema** out) {
   if (!out || n_fields < 0 || (n_fields > 0 && !fields)) return fail(TFR_E_INVALID_ARG, "null argument");
-  if (schema_flags & ~TFR_S_RAGGED) return fail(TFR_E_INVALID_ARG, "unknown schema flags");
+  if (schema_flags & ~(TFR_S_RAGGED | TFR_S_INT64_TYPES)) return fail(TFR_E_INVALID_ARG, "unknown schema flags");
   if (record_type < TFR_RT_EXAMPLE || record_type > TFR_RT_BYTE_ARRAY)
     return fail(TFR_E_BAD_RECORD_TYPE, "Unsupported recordType: recordType can be ByteArray, Example or SequenceExample");
   if ((schema_flags & TFR_S_RAGGED) && record_type == TFR_RT_SEQUENCE_EXAMPLE)
@@ -285,6 +295,7 @@ extern "C" int32_t tfr_schema_create_ex(const tfr_field* fields, int32_t n_field
     s->vec.assign(s->fields.size(), VK_NONE);
     s->part.assign(s->fields.size(), -1);
     s->rag_len.assign(s->fields.size(), -1);
+    s->nar.assign(s->fields.size(), 0);
     s->n_user = (int32_t)s->fields.size();
     *out = s.release();
     return TFR_OK;
@@ -311,6 +322,7 @@ extern "C" int32_t tfr_schema_create_ex(const tfr_field* fields, int32_t n_field
     s->vec.push_back(vk);
     s->part.push_back(part);
     s->rag_len.push_back(-1);
+    s->nar.push_back(0);
   };
   std::vector<std::string> user(n_fields);              // the caller's names
   std::vector<int32_t> sparse, ragged;                  // the sparse vectors and the ragged fields, in field order
@@ -320,12 +332,16 @@ extern "C" int32_t tfr_schema_create_ex(const tfr_field* fields, int32_t n_field
     std::string nm(f.name ? f.name : "", (size_t)f.name_len);
     user[i] = nm;
     int32_t rc = TFR_OK;
-    if (add_generated(*s, f, nm, &rc)) { if (rc) return rc; s->vec.push_back(VK_NONE); s->part.push_back(-1); s->rag_len.push_back(-1); continue; }
+    if (add_generated(*s, f, nm, &rc)) { if (rc) return rc; s->vec.push_back(VK_NONE); s->part.push_back(-1); s->rag_len.push_back(-1); s->nar.push_back(0); continue; }
     // a VectorUDT field is an ArrayType(DoubleType) field to every kernel but the UnsafeRow ones (VECTORS); a sparse one is
     // its values field here, and its indices and size fields are appended below (SPARSE VECTORS)
     const bool vector = f.elem_type == TFR_T_VECTOR, sp = f.elem_type == TFR_T_SPARSE_VECTOR;
     if ((vector || sp) && f.depth != 0) return fail(TFR_E_UNSUPPORTED_TYPE, "field '" + nm + "': ArrayType(VectorUDT) is not supported");
-    const int32_t et = vector || sp ? TFR_T_FLOAT64 : f.elem_type, depth = vector || sp ? 1 : f.depth;
+    // a BooleanType .. TimestampType field is a LongType field to every kernel but narrow.cuh's (INT64 TYPES)
+    const bool i64t = nar_width(f.elem_type) > 0;
+    if (i64t && !(schema_flags & TFR_S_INT64_TYPES))
+      return fail(TFR_E_UNSUPPORTED_TYPE, "field '" + nm + "': data type is not supported (Boolean, Byte, Short, Date and Timestamp need extendedTypes=true)");
+    const int32_t et = vector || sp ? TFR_T_FLOAT64 : i64t ? TFR_T_INT64 : f.elem_type, depth = vector || sp ? 1 : f.depth;
     // newFeatureWriter / newFeatureConverter: anything but these types throws (M/TFRecordDeserializer.scala:119-123,
     // M/TFRecordSerializer.scala:147,151); ArrayType(NullType) falls into the same default branch
     bool ok_type = et >= TFR_T_NULL && et <= TFR_T_BINARY && depth >= 0 && depth <= 2 && !(et == TFR_T_NULL && depth > 0);
@@ -336,6 +352,7 @@ extern "C" int32_t tfr_schema_create_ex(const tfr_field* fields, int32_t n_field
     if (rg) ragged.push_back(i);
     add(sp ? nm + TFR_SPARSE_VALUES_SUFFIX : rg ? nm + TFR_RAGGED_VALUES_SUFFIX : nm, et, rg ? 1 : depth, f.nullable != 0,
         vector ? VK_DENSE : sp ? VK_SPARSE : VK_NONE, -1);
+    if (i64t) s->nar.back() = (int8_t)f.elem_type;
   }
   s->n_user = n_fields;
   for (int32_t v : sparse) {
@@ -350,7 +367,7 @@ extern "C" int32_t tfr_schema_create_ex(const tfr_field* fields, int32_t n_field
   s->n_rag = (int32_t)ragged.size();
   if (s->n_rag) {
     tfr_schema* p = nullptr;
-    TRY(tfr_schema_create_ex(fields, n_fields, record_type, 0, &p));
+    TRY(tfr_schema_create_ex(fields, n_fields, record_type, schema_flags & TFR_S_INT64_TYPES, &p));
     s->plain.reset(p);
   }
   // Spark refuses duplicate column names for file sources before the reader is built
@@ -398,12 +415,14 @@ extern "C" int32_t tfr_schema_num_fields(const tfr_schema* s) { return s ? s->n_
 struct DevSchemaBuf {
   DevBuf fields, names, ht, var_field, templates;
   DevBuf vec, part;                                       // tfr_schema::vec and ::part, for the UnsafeRow kernels of the encoder
+  DevBuf nar;                                             // tfr_schema::nar, for the same kernels (INT64 TYPES)
   DevBuf rag; int32_t n_rag = 0;                          // pairs (ragged field, its lengths part), for decode_pass1_kernel<true>
   DevBuf tile_consts; uint32_t tile_consts_bytes = 0;     // tile.cuh: per-schema constants in the shared-memory layout
   DevSchema view{};
   const int32_t* d_var_field() const { return (const int32_t*)var_field.p; }
   const uint8_t* d_vec() const { return (const uint8_t*)vec.p; }
   const int32_t* d_part() const { return (const int32_t*)part.p; }
+  const int8_t* d_nar() const { return (const int8_t*)nar.p; }
   const uint8_t* d_tile_consts() const { return (const uint8_t*)tile_consts.p; }
   // `unkeyed`: a field no feature maps to (schema_rehash), which gets no entry template either
   int32_t upload(const tfr_schema& s, cudaStream_t st, int32_t unkeyed = -1) {
@@ -414,6 +433,8 @@ struct DevSchemaBuf {
     CUDA_TRY(var_field.alloc(std::max<size_t>(1, s.var_field.size()) * sizeof(int32_t)));
     CUDA_TRY(vec.alloc(std::max<size_t>(1, nf)));
     CUDA_TRY(part.alloc(std::max<size_t>(1, nf) * sizeof(int32_t)));
+    CUDA_TRY(nar.alloc(std::max<size_t>(1, nf)));
+    if (!s.nar.empty()) CUDA_TRY(cudaMemcpyAsync(nar.p, s.nar.data(), s.nar.size(), cudaMemcpyHostToDevice, st));
     if (nf) CUDA_TRY(cudaMemcpyAsync(fields.p, s.fields.data(), nf * sizeof(DevField), cudaMemcpyHostToDevice, st));
     if (!s.vec.empty()) CUDA_TRY(cudaMemcpyAsync(vec.p, s.vec.data(), s.vec.size(), cudaMemcpyHostToDevice, st));
     if (!s.part.empty()) CUDA_TRY(cudaMemcpyAsync(part.p, s.part.data(), s.part.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
@@ -526,6 +547,8 @@ static const char* leaf_format(int t) {
   switch (t) {
     case TFR_T_INT32: return "i"; case TFR_T_INT64: return "l"; case TFR_T_FLOAT32: return "f";
     case TFR_T_FLOAT64: case TFR_T_DECIMAL: return "g"; case TFR_T_STRING: return "u"; case TFR_T_BINARY: return "z";
+    case TFR_T_BOOL: return "b"; case TFR_T_INT8: return "c"; case TFR_T_INT16: return "s"; case TFR_T_DATE: return "tdD";
+    case TFR_T_TIMESTAMP: return "tsu:UTC";
     default: return "n";
   }
 }
@@ -538,8 +561,9 @@ static void build_schema(ArrowSchema* s, const char* name, int elem_type, int de
   s->children[0] = new ArrowSchema;
   build_schema(s->children[0], "item", elem_type, depth - 1);
 }
-// level: which offsets level this list node uses; leaves use the last level for utf8/binary
-static void build_array(ArrowArray* a, const tfr_column& c, int level, int64_t length, tfr_batch* owner) {
+// level: which offsets level this list node uses; leaves use the last level for utf8/binary.  bits: a boolean column's bit-packed
+// values (INT64 TYPES), which its leaf hands out in place of the bytes of c.values
+static void build_array(ArrowArray* a, const tfr_column& c, int level, int64_t length, tfr_batch* owner, const void* bits = nullptr) {
   memset(a, 0, sizeof *a);
   auto* p = new ExportPriv;
   p->batch = owner;
@@ -555,14 +579,14 @@ static void build_array(ArrowArray* a, const tfr_column& c, int level, int64_t l
     p->children.resize(1); p->children[0] = new ArrowArray;
     a->children = p->children.data();
     int64_t child_len = level + 1 < c.n_levels ? c.n_offsets[level + 1] - 1 : c.n_values;
-    build_array(a->children[0], c, level + 1, child_len, nullptr);
+    build_array(a->children[0], c, level + 1, child_len, nullptr, bits);
   } else if (c.elem_type == TFR_T_NULL) {
     a->n_buffers = 0; a->null_count = length;
   } else if (varlen) {
     p->buffers = {validity, c.offsets[c.n_levels - 1], c.values};
     a->n_buffers = 3;
   } else {
-    p->buffers = {validity, c.values};
+    p->buffers = {validity, c.elem_type == TFR_T_BOOL ? bits : c.values};
     a->n_buffers = 2;
   }
   a->buffers = p->buffers.data();
@@ -577,7 +601,8 @@ extern "C" int32_t tfr_batch_export_arrow_host(tfr_batch* b, int32_t column, voi
   std::string nm((const char*)&S.names[S.fields[column].name_off], S.fields[column].name_len);
   if (S.ragged(column)) nm.resize(nm.size() - strlen(TFR_RAGGED_VALUES_SUFFIX));     // x, not its values part's key
   build_schema((ArrowSchema*)arrow_schema, nm.c_str(), c.elem_type, c.depth);
-  build_array((ArrowArray*)arrow_array, c, 0, c.n_rows, b);
+  const void* bits = c.elem_type == TFR_T_BOOL ? b->out.host_ptr((uint8_t*)b->host_copy.block.get(), b->out.bool_bits((uint32_t)column)) : nullptr;
+  build_array((ArrowArray*)arrow_array, c, 0, c.n_rows, b, bits);
   return TFR_OK;
 }
 extern "C" int32_t tfr_batch_export_arrow_device(tfr_batch* b, int32_t column, void* arrow_device_array, void* arrow_schema) {
@@ -591,7 +616,7 @@ extern "C" int32_t tfr_batch_export_arrow_device(tfr_batch* b, int32_t column, v
   build_schema((ArrowSchema*)arrow_schema, nm.c_str(), c.elem_type, c.depth);
   auto* da = (ArrowDeviceArray*)arrow_device_array;
   memset(da, 0, sizeof *da);
-  build_array(&da->array, c, 0, c.n_rows, b);
+  build_array(&da->array, c, 0, c.n_rows, b, c.elem_type == TFR_T_BOOL ? b->out.bool_bits((uint32_t)column) : nullptr);
   da->device_id = b->dec->device; da->device_type = 2 /*ARROW_DEVICE_CUDA*/; da->sync_event = nullptr;   // batch already waited
   return TFR_OK;
 }

@@ -22,6 +22,7 @@
 #include "common.cuh"
 #include "encode.cuh"
 #include "tile.cuh"
+#include "narrow.cuh"
 
 #define ROWS_TILE 32
 #define ROWS_B_WARPS 4
@@ -44,6 +45,8 @@ struct RowsArgs {
   const int32_t* part;          // [n_fields] VK_SPARSE: the field of its indices (its size's follows)
   uint32_t nu;                  // the rows' fields: the schema's but a sparse vector's parts, which are filled with it
 };
+// The NW instantiations of pass A and B take, beside RowsArgs, `nar`: [n_fields] a BooleanType .. TimestampType field's TFR_T_*
+// (include/tfrgpu.h, INT64 TYPES), else 0.
 
 enum { RW_OK = 0, RW_NULL = 1, RW_BAD = 2 };
 
@@ -74,15 +77,38 @@ __device__ __forceinline__ bool rows_var_elem(const uint8_t* row, uint64_t a, ui
 }
 __device__ __forceinline__ bool rows_is_var(const DevField& fd) { return fd.elem_type == TFR_T_STRING || fd.elem_type == TFR_T_BINARY; }
 
+// INT64 TYPES: the int64 a row's value of type nt writes, from its slot or element bits (UnsafeRow.getBoolean is a byte != 0;
+// getByte, getShort and getInt sign-extend; a timestamp is its long)
+__device__ __forceinline__ long long rows_widen(int nt, uint64_t bits) {
+  switch (nt) {
+    case TFR_T_BOOL: return (bits & 0xffu) != 0 ? 1 : 0;
+    case TFR_T_INT8: return (long long)(int8_t)bits;
+    case TFR_T_INT16: return (long long)(int16_t)bits;
+    case TFR_T_DATE: return (long long)(int32_t)bits;
+    default: return (long long)bits;
+  }
+}
+// element i of an UnsafeArrayData of type nt whose element slots start at row byte d (1, 1, 2, 4 or 8 bytes wide)
+__device__ __forceinline__ uint64_t rows_narrow_elem(const uint8_t* row, uint64_t d, int nt, uint32_t i) {
+  switch (nar_width(nt)) {
+    case 1: return row[d + i];
+    case 2: return reinterpret_cast<const uint16_t*>(row + d)[i];
+    case 4: return reinterpret_cast<const uint32_t*>(row + d)[i];
+    default: return rows_ld64(row + d + 8ull * i);
+  }
+}
+
 // Counts of one non-null variable-width field: c[l] = the entries this row adds to offsets level l (level 0: bytes,
 // elements or steps; deeper levels: their children).  `room` grows by the value bytes plus 8 per inner-level entry: a
 // well-formed row spends at least that much of its own bytes on them, which bounds the column buffers by the input.
-__device__ int rows_field_counts(const uint8_t* row, uint64_t len, const DevField& fd, uint64_t slot, uint32_t c[3], uint64_t& room) {
+// NW: nt is an INT64 TYPES field's TFR_T_* (0 none), whose array elements are nar_width(nt) bytes wide in the row.
+template <bool NW>
+__device__ int rows_field_counts(const uint8_t* row, uint64_t len, const DevField& fd, uint64_t slot, uint32_t c[3], uint64_t& room, int nt) {
   const uint64_t o = slot >> 32, sz = slot & 0xffffffffu;
   if ((o & 7) || o + sz > len) return RW_BAD;
   const bool var = rows_is_var(fd);
   if (fd.depth == 0) { c[0] = (uint32_t)sz; room += sz; return RW_OK; }
-  const uint32_t esz = var ? 8u : (uint32_t)fd.width;      // int/float 4, long/double/decimal 8
+  const uint32_t esz = var ? 8u : NW && nt ? (uint32_t)nar_width(nt) : (uint32_t)fd.width;      // int/float 4, long/double/decimal 8
   const bool null_elem_is_error = var || fd.elem_type == TFR_T_DECIMAL;   // getUTF8String / getBinary / getDecimal of a null (:118-135)
   uint32_t n;
   uint64_t d;
@@ -171,9 +197,10 @@ __device__ int rows_vector(const uint8_t* row, uint64_t len, uint64_t slot, bool
 // from the scanned counts, so they add nothing to `room`.  A sparse-format vector's toSparse entries are counted by pass A
 // itself (rows_sparse_count); they number no more than its stored values, which `room` takes at 8 bytes each, so its values
 // are bounded by the input like a double array's and its int32 indices by half of that (rows_layout sizes the arena so).
+template <bool NW>
 __device__ __forceinline__ int rows_counts(const RowsArgs& A, uint32_t f, const uint8_t* row, uint64_t len, const DevField& fd, uint64_t slot,
-                                           uint32_t c[3], uint64_t& room) {
-  if (A.vec[f] == VK_NONE) return rows_field_counts(row, len, fd, slot, c, room);
+                                           uint32_t c[3], uint64_t& room, const int8_t* nar) {
+  if (A.vec[f] == VK_NONE) return rows_field_counts<NW>(row, len, fd, slot, c, room, NW ? nar[f] : 0);
   RowsVec v;
   if (rows_vector(row, len, slot, true, v) != RW_OK) return RW_BAD;
   c[0] = v.size;
@@ -212,7 +239,9 @@ __device__ __forceinline__ uint32_t rows_sparse_count(const uint8_t* row, uint64
 
 __device__ __forceinline__ bool rows_field_null(const uint8_t* row, uint32_t f) { return (rows_ld64(row + 8ull * (f >> 6)) >> (f & 63)) & 1; }
 
-__global__ void __launch_bounds__(ROWS_TILE) rows_pass_a_kernel(RowsArgs A) {
+// NW: the schema has a BooleanType .. DateType field (nar); NW = false is the kernel of every other schema and never reads nar.
+template <bool NW>
+__global__ void __launch_bounds__(ROWS_TILE) rows_pass_a_kernel(RowsArgs A, const int8_t* nar) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw);
   uint8_t* tile_b = smem_raw + 16;
@@ -256,7 +285,7 @@ __global__ void __launch_bounds__(ROWS_TILE) rows_pass_a_kernel(RowsArgs A) {
       const DevField& fd = A.sch.fields[f];
       if (fd.n_levels == 0 || rows_field_null(row, f)) continue;
       uint32_t c[3];
-      const int st = rows_counts(A, f, row, len, fd, rows_ld64(row + 8ull * (nw + f)), c, room);
+      const int st = rows_counts<NW>(A, f, row, len, fd, rows_ld64(row + 8ull * (nw + f)), c, room, nar);
       if (st == RW_BAD) { bad = true; break; }
       if (st == RW_NULL) nul = true;
     }
@@ -288,6 +317,7 @@ __global__ void __launch_bounds__(ROWS_TILE) rows_pass_a_kernel(RowsArgs A) {
     if (fd.n_levels == 0) {
       const uint64_t s = present ? rows_ld64(row + 8ull * (nw + f)) : 0;
       void* v = A.fixv[f];
+      if (NW && nar[f]) { reinterpret_cast<long long*>(v)[r] = rows_widen(nar[f], s); continue; }   // a null's 0 widens to 0
       if (fd.width == 4) reinterpret_cast<uint32_t*>(v)[r] = (uint32_t)s;                      // IntegerType / FloatType: the low 4 bytes
       else if (fd.elem_type == TFR_T_DECIMAL)                                                    // BigDecimal(v, 0).floatValue, carried as float64
         reinterpret_cast<double*>(v)[r] = present ? (double)__ll2float_rn((long long)s) : 0.0;
@@ -296,7 +326,7 @@ __global__ void __launch_bounds__(ROWS_TILE) rows_pass_a_kernel(RowsArgs A) {
     }
     uint32_t c[3] = {0, 0, 0};
     uint64_t room = 0;
-    if (present) rows_counts(A, f, row, len, fd, rows_ld64(row + 8ull * (nw + f)), c, room);
+    if (present) rows_counts<NW>(A, f, row, len, fd, rows_ld64(row + 8ull * (nw + f)), c, room, nar);
     for (int l = 0; l < fd.n_levels; ++l) A.cnt[(size_t)(fd.cnt_slot + l) * A.n_rows + r] = c[l];
   }
 }
@@ -392,9 +422,14 @@ __device__ __forceinline__ void rows_copy(uint8_t* dst, const uint8_t* src, uint
     for (uint32_t o = lane * 64; o < k; o += 32 * 64) rows_copy_lane(d + o, s + o, min(64u, k - o));
   }
 }
-// numeric elements [i0, i0 + m) of the array whose slots start at row byte d -> column values from index `at`
-__device__ __forceinline__ void rows_copy_elems(const DevField& fd, void* values, uint64_t at, const uint8_t* row, uint64_t d, uint32_t m) {
-  if (fd.width == 4) {
+// numeric elements [i0, i0 + m) of the array whose slots start at row byte d -> column values from index `at`.  NW: nt is an INT64
+// TYPES field's TFR_T_* (0 none), whose elements widen into the int64 column (a null element: its slot's bits, as LongType's).
+template <bool NW>
+__device__ __forceinline__ void rows_copy_elems(const DevField& fd, void* values, uint64_t at, const uint8_t* row, uint64_t d, uint32_t m, int nt) {
+  if (NW && nt) {
+    long long* v = reinterpret_cast<long long*>(values) + at;
+    for (uint32_t i = 0; i < m; ++i) v[i] = rows_widen(nt, rows_narrow_elem(row, d, nt, i));
+  } else if (fd.width == 4) {
     uint32_t* v = reinterpret_cast<uint32_t*>(values) + at;
     const uint32_t* s = reinterpret_cast<const uint32_t*>(row + d);
     for (uint32_t i = 0; i < m; ++i) v[i] = s[i];                    // a null element keeps its slot's bits (toIntArray / toFloatArray)
@@ -479,7 +514,8 @@ __device__ __forceinline__ void rows_sparse_fill(const uint8_t* row, uint64_t sl
   }
 }
 
-__global__ void __launch_bounds__(ROWS_B_WARPS * 32) rows_pass_b_kernel(RowsArgs A) {
+template <bool NW>
+__global__ void __launch_bounds__(ROWS_B_WARPS * 32) rows_pass_b_kernel(RowsArgs A, const int8_t* nar) {
   if (A.st->rows_overflow) return;                                   // the columns were not placed: nothing to fill
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t w = blockIdx.x * ROWS_B_WARPS + (threadIdx.x >> 5);
@@ -506,12 +542,13 @@ __global__ void __launch_bounds__(ROWS_B_WARPS * 32) rows_pass_b_kernel(RowsArgs
     if (fd.depth == 0) { rows_copy(values + e0, row + o, (uint32_t)sz, v); continue; }
     if (!v) continue;
     const bool var = rows_is_var(fd);
-    const uint32_t esz = var ? 8u : (uint32_t)fd.width;
+    const int nt = NW ? nar[f] : 0;
+    const uint32_t esz = var ? 8u : NW && nt ? (uint32_t)nar_width(nt) : (uint32_t)fd.width;
     uint32_t n;
     uint64_t d, eo, es;
     rows_array(row, o, sz, fd.depth == 2 ? 8u : esz, n, d);
     if (fd.depth == 1) {
-      if (!var) { rows_copy_elems(fd, values, (uint64_t)e0, row, d, n); continue; }
+      if (!var) { rows_copy_elems<NW>(fd, values, (uint64_t)e0, row, d, n, nt); continue; }
       int32_t* o1 = const_cast<int32_t*>(c.off[1]);
       int32_t b = A.lev[fd.cnt_slot + 1][r];
       for (uint32_t i = 0; i < n; ++i) {
@@ -532,7 +569,7 @@ __global__ void __launch_bounds__(ROWS_B_WARPS * 32) rows_pass_b_kernel(RowsArgs
       uint32_t m;
       uint64_t d2, fo, fs;
       rows_array(row, eo, es, esz, m, d2);
-      if (!var) { rows_copy_elems(fd, values, (uint64_t)b1, row, d2, m); b1 += (int32_t)m; continue; }
+      if (!var) { rows_copy_elems<NW>(fd, values, (uint64_t)b1, row, d2, m, nt); b1 += (int32_t)m; continue; }
       for (uint32_t j = 0; j < m; ++j) {
         rows_var_elem(row, eo, es, d2, j, fo, fs);
         o2[b1 + j] = b2;

@@ -42,7 +42,9 @@
 // UR_VEC: a VectorUDT field (include/tfrgpu.h, VECTORS), a float64 list column written as the nested row of a dense vector.
 // UR_SVEC: a sparse-vector field (SPARSE VECTORS), its values column written with its indices and size columns (cols[part],
 // cols[part + 1], which are not row fields of their own) as the nested row of a sparse vector.
-enum { UR_NULL = 0, UR_FIX4 = 1, UR_FIX8 = 2, UR_BYTES = 3, UR_ARR = 4, UR_ARR2 = 5, UR_VEC = 6, UR_SVEC = 7 };
+// UR_FIX1, UR_FIX2: a BooleanType / ByteType or ShortType scalar (include/tfrgpu.h, INT64 TYPES), whose arrays have 1- and 2-byte
+// elements.  Only the emit kernel's NW instantiation writes them; NW = false is the kernel of every other schema.
+enum { UR_NULL = 0, UR_FIX4 = 1, UR_FIX8 = 2, UR_BYTES = 3, UR_ARR = 4, UR_ARR2 = 5, UR_VEC = 6, UR_SVEC = 7, UR_FIX1 = 8, UR_FIX2 = 9 };
 #define UR_VEC_HEAD 40u         // the nested row's fixed part: one null word and four slots
 
 struct UrCol {                  // one decoded column (tfr_column), device pointers
@@ -50,7 +52,7 @@ struct UrCol {                  // one decoded column (tfr_column), device point
   const int32_t* off[3];        // offsets levels
   const uint8_t* values;
   int32_t kind;                 // UR_*
-  int32_t width;                // leaf bytes of a numeric leaf (4 / 8); 0 for string / binary leaves
+  int32_t width;                // leaf bytes of a numeric leaf (1 / 2 / 4 / 8); 0 for string / binary leaves
   int32_t var;                  // index among the variable-width fields (UR_BYTES, UR_ARR, UR_ARR2, UR_VEC, UR_SVEC), -1 otherwise
   int32_t part;                 // UR_SVEC: the column of its indices (its size's follows), 0 otherwise
 };
@@ -146,9 +148,14 @@ __device__ __forceinline__ void ur_copy_bytes(uint8_t* dst, const uint8_t* src, 
   for (uint64_t k = 8ull * k0; k < n; k += 8ull * step)
     *reinterpret_cast<unsigned long long*>(dst + k) = ur_gather8(src + k, n - k);
 }
-// m numeric leaves of width w (4 / 8, w-aligned source) to an 8-byte aligned destination
+// m numeric leaves of width w (4 / 8, and with NW 1 / 2; w-aligned source) to an 8-byte aligned destination
+template <bool NW>
 __device__ __forceinline__ void ur_copy_elems(uint8_t* dst, const uint8_t* src, uint64_t m, int w, uint32_t k0, uint32_t step) {
-  if (w == 4) {
+  if (NW && w == 1) {
+    for (uint64_t i = k0; i < m; i += step) dst[i] = src[i];
+  } else if (NW && w == 2) {
+    for (uint64_t i = k0; i < m; i += step) reinterpret_cast<uint16_t*>(dst)[i] = reinterpret_cast<const uint16_t*>(src)[i];
+  } else if (w == 4) {
     for (uint64_t i = k0; i < m; i += step) reinterpret_cast<uint32_t*>(dst)[i] = reinterpret_cast<const uint32_t*>(src)[i];
   } else {
     for (uint64_t i = k0; i < m; i += step) reinterpret_cast<unsigned long long*>(dst)[i] = reinterpret_cast<const unsigned long long*>(src)[i];
@@ -181,16 +188,17 @@ __device__ void ur_emit_svec(const UrCol& c, const UrCol* cols, uint32_t r, uint
     ur_st64(dst + 32, (vo << 32) | ur_arr1_bytes(c, 0, a, b));
     ur_st64(dst + vo, m);
   }
-  if (ip) ur_copy_elems(dst + UR_VEC_HEAD + ur_hdr(mi), ci.values + (uint64_t)ia * 4, mi, 4, k0, step);
-  ur_copy_elems(dst + vo + ur_hdr(m), c.values + (uint64_t)a * 8, m, 8, k0, step);
+  if (ip) ur_copy_elems<false>(dst + UR_VEC_HEAD + ur_hdr(mi), ci.values + (uint64_t)ia * 4, mi, 4, k0, step);
+  ur_copy_elems<false>(dst + vo + ur_hdr(m), c.values + (uint64_t)a * 8, m, 8, k0, step);
 }
 
 // one lane writes the 1-D array of elements [e0, e1) of level lvl + 1 at dst (zeroed); returns its bytes
+template <bool NW>
 __device__ uint64_t ur_emit_arr1_lane(const UrCol& c, int lvl, int64_t e0, int64_t e1, uint8_t* dst) {
   const uint64_t m = (uint64_t)(e1 - e0), h = ur_hdr(m);
   ur_st64(dst, m);                                                           // the element null bitset stays zero
   if (c.width) {
-    ur_copy_elems(dst + h, c.values + (uint64_t)e0 * c.width, m, c.width, 0, 1);
+    ur_copy_elems<NW>(dst + h, c.values + (uint64_t)e0 * c.width, m, c.width, 0, 1);
     return h + ur_pad8(m * (uint64_t)c.width);
   }
   const int32_t* o = c.off[lvl + 1];
@@ -213,6 +221,7 @@ __device__ __forceinline__ uint64_t ur_warp_scan(uint64_t x) {
 }
 
 // the whole warp writes row r's value of field c at dst (zeroed); warp-uniform call
+template <bool NW>
 __device__ void ur_emit_warp(const UrCol& c, uint32_t r, uint8_t* dst) {
   const uint32_t lane = threadIdx.x & 31;
   const int64_t a = c.off[0][r], b = c.off[0][r + 1];
@@ -223,7 +232,7 @@ __device__ void ur_emit_warp(const UrCol& c, uint32_t r, uint8_t* dst) {
     dst += UR_VEC_HEAD;
   }
   if (lane == 0) ur_st64(dst, m);
-  if ((c.kind == UR_ARR || c.kind == UR_VEC) && c.width) { ur_copy_elems(dst + h, c.values + (uint64_t)a * c.width, m, c.width, lane, 32); return; }
+  if ((c.kind == UR_ARR || c.kind == UR_VEC) && c.width) { ur_copy_elems<NW>(dst + h, c.values + (uint64_t)a * c.width, m, c.width, lane, 32); return; }
   // elements with an (offset << 32 | size) slot each: strings / binaries (UR_ARR) or inner arrays (UR_ARR2).  32 at a time,
   // each lane sizes its element, a scan places them, each lane writes its element
   uint64_t base = h + 8 * m;
@@ -236,23 +245,24 @@ __device__ void ur_emit_warp(const UrCol& c, uint32_t r, uint8_t* dst) {
     if (on) {
       ur_st64(dst + h + 8 * (uint64_t)(k - a), (p << 32) | len);
       if (c.kind == UR_ARR) ur_copy_bytes(dst + p, c.values + c.off[1][k], len, 0, 1);
-      else ur_emit_arr1_lane(c, 1, c.off[1][k], c.off[1][k + 1], dst + p);
+      else ur_emit_arr1_lane<NW>(c, 1, c.off[1][k], c.off[1][k + 1], dst + p);
     }
     base += __shfl_sync(FULLMASK, incl, 31);
   }
 }
 
 // one lane writes row r's value of field c at dst (zeroed)
+template <bool NW>
 __device__ void ur_emit_lane(const UrCol& c, uint32_t r, uint8_t* dst) {
   const int64_t a = c.off[0][r], b = c.off[0][r + 1];
   if (c.kind == UR_BYTES) { ur_copy_bytes(dst, c.values + a, (uint64_t)(b - a), 0, 1); return; }
-  if (c.kind == UR_ARR) { ur_emit_arr1_lane(c, 0, a, b, dst); return; }
-  if (c.kind == UR_VEC) { ur_vec_head(dst, ur_emit_arr1_lane(c, 0, a, b, dst + UR_VEC_HEAD)); return; }
+  if (c.kind == UR_ARR) { ur_emit_arr1_lane<NW>(c, 0, a, b, dst); return; }
+  if (c.kind == UR_VEC) { ur_vec_head(dst, ur_emit_arr1_lane<NW>(c, 0, a, b, dst + UR_VEC_HEAD)); return; }
   const uint64_t m = (uint64_t)(b - a), h = ur_hdr(m);
   ur_st64(dst, m);
   uint64_t p = h + 8 * m;
   for (int64_t k = a; k < b; ++k) {
-    const uint64_t len = ur_emit_arr1_lane(c, 1, c.off[1][k], c.off[1][k + 1], dst + p);
+    const uint64_t len = ur_emit_arr1_lane<NW>(c, 1, c.off[1][k], c.off[1][k + 1], dst + p);
     ur_st64(dst + h + 8 * (uint64_t)(k - a), (p << 32) | len);
     p += len;
   }
@@ -270,8 +280,8 @@ __global__ void urows_verdict_kernel(uint32_t* ctl, const uint64_t* total, uint3
 
 // GUARD: the asynchronous pass's instantiation.  It returns at once when urows_verdict_kernel has raised the verdict, takes the
 // row count from ctl[URC_N] (A.n_rows is the capacity, the stride of `pos`), and CTAs past the count exit.  GUARD = false never
-// reads `ctl`.
-template <bool GUARD>
+// reads `ctl`.  NW: the schema has a field of a 1- or 2-byte type (UR_FIX1, UR_FIX2).
+template <bool GUARD, bool NW>
 __global__ void __launch_bounds__(UROWS_WARPS * 32) urows_emit_kernel(UrArgs A, const uint32_t* ctl) {
   extern __shared__ __align__(16) uint8_t ur_smem[];
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -302,6 +312,10 @@ __global__ void __launch_bounds__(UROWS_WARPS * 32) urows_emit_kernel(UrArgs A, 
     const bool present = act && ((vw >> lane) & 1u);
     if (act && !present) atomicOr(reinterpret_cast<unsigned long long*>(row + 8ull * (f >> 6)), 1ull << (f & 63));
     uint8_t* slot = row + 8ull * (A.nw + f);
+    if (NW && (c.kind == UR_FIX1 || c.kind == UR_FIX2)) {            // the slot zeroed, then 1 or 2 bytes
+      if (present) ur_st64(slot, c.kind == UR_FIX1 ? (uint64_t)c.values[r] : (uint64_t)reinterpret_cast<const uint16_t*>(c.values)[r]);
+      continue;
+    }
     if (c.kind == UR_FIX4 || c.kind == UR_FIX8) {
       if (present) ur_st64(slot, c.kind == UR_FIX4 ? (uint64_t)reinterpret_cast<const uint32_t*>(c.values)[r]
                                                    : (uint64_t)reinterpret_cast<const unsigned long long*>(c.values)[r]);
@@ -315,14 +329,14 @@ __global__ void __launch_bounds__(UROWS_WARPS * 32) urows_emit_kernel(UrArgs A, 
       ur_st64(slot, (p << 32) | len);
     }
     const bool big = present && ur_pad8(len) >= UROWS_BIG;
-    if (present && !big) { if (c.kind == UR_SVEC) ur_emit_svec(c, A.cols, r, row + p, 0, 1); else ur_emit_lane(c, r, row + p); }
+    if (present && !big) { if (c.kind == UR_SVEC) ur_emit_svec(c, A.cols, r, row + p, 0, 1); else ur_emit_lane<NW>(c, r, row + p); }
     uint32_t mb = __ballot_sync(FULLMASK, big);
     while (mb) {
       const int l = __ffs(mb) - 1;
       mb &= mb - 1;
       uint8_t* d = (uint8_t*)__shfl_sync(FULLMASK, (unsigned long long)(row + p), l);
       if (c.kind == UR_SVEC) ur_emit_svec(c, A.cols, r0 + (uint32_t)l, d, lane, 32);
-      else ur_emit_warp(c, r0 + (uint32_t)l, d);
+      else ur_emit_warp<NW>(c, r0 + (uint32_t)l, d);
     }
   }
   // ---- the partition values: lane = row, warp w takes units w, w + UROWS_WARPS, ... of [the null words holding partition

@@ -83,6 +83,16 @@ def _nested_array_format(options: Optional[Dict[str, str]]) -> bool:
     return nf == "ragged"
 
 
+def _extended_types(options: Optional[Dict[str, str]]) -> bool:
+    """the `extendedTypes` option: "true" reads and writes BooleanType, ByteType, ShortType, DateType and TimestampType fields
+    (and arrays of them) as Int64 features (include/tfrgpu.h, INT64 TYPES); "false" (the default) refuses them, as the
+    reference does.  Anything else is refused before any work."""
+    value = (options or {}).get("extendedTypes", "false")
+    if value not in ("true", "false"):
+        raise _native.IllegalArgumentException(-1, f"extendedTypes {value}: the option takes true or false")
+    return value == "true"
+
+
 def _corrupt_column_name(options: Optional[Dict[str, str]]) -> str:
     """the option columnNameOfCorruptRecord, named and defaulted as Spark's JSON and CSV sources have it"""
     return (options or {}).get("columnNameOfCorruptRecord", "_corrupt_record")
@@ -484,12 +494,14 @@ class TFRecordFileReader:
         rt = _record_type(options)
         vf = _vector_format(options)
         ragged = _nested_array_format(options)
+        ext = _extended_types(options)
         flags, corrupt = _read_mode(options, schema if dataSchema is None else dataSchema, schema)
         block = block_bytes or TFRecordFileReader.BLOCK_BYTES
         # recordIndex=true: a split of a file reads exactly the frames whose header offset lies in it (RECORD INDEX)
         split = (_record_index(options) and _codec_of_path(file.toPath()) is None
                  and (file.start, file.length) != (0, os.path.getsize(file.toPath())))
-        dec = _native.Decoder(_decoder_schema(schema), rt, device, flags, corrupt_field=corrupt, vector_format=vf, ragged=ragged)
+        dec = _native.Decoder(_decoder_schema(schema), rt, device, flags, corrupt_field=corrupt, vector_format=vf, ragged=ragged,
+                              extended_types=ext)
 
         def gen():
             todo = []
@@ -598,7 +610,7 @@ class TFRecordOutputWriter:
         self.schema = byte_array_schema() if self.recordType == 2 else dataSchema
         self.vectorFormat = _vector_format(options)
         self._enc = _native.Encoder(self.schema, self.recordType, device, vector_format=self.vectorFormat,
-                                    ragged=_nested_array_format(options))
+                                    ragged=_nested_array_format(options), extended_types=_extended_types(options))
         self._rows: List[tuple] = []
         self._bytes = 0
         codec = _codec_name((options or {}).get("codec", ""))
@@ -725,6 +737,7 @@ class DefaultSource:
         reads the files back under the options it was inferred with (buildReader refuses PERMISSIVE without it)."""
         from .sharding import allreduce_schema, codes_to_struct, shard_lpt
         _nested_array_format(options)                 # validated; a ragged file infers as its two plain fields
+        _extended_types(options)                      # validated; an Int64List still infers as LongType
         mode, flags = _mode_flags(options)
         rt = _record_type(options)
         if rt == 2:
@@ -785,6 +798,7 @@ class DefaultSource:
         _read_mode(options, dataSchema, requiredSchema)
         _vector_format(options)
         _nested_array_format(options)
+        _extended_types(options)
         _record_index(options)
         return lambda file: TFRecordFileReader.readFile(None, options, file, requiredSchema, device, dataSchema=dataSchema)
 
@@ -792,6 +806,7 @@ class DefaultSource:
         codec = _codec_name((options or {}).get("codec", ""))             # :94-102: the option turns output compression on
         _vector_format(options)
         _nested_array_format(options)
+        _extended_types(options)
         _check_record_index(options, codec)
 
         class _Factory:

@@ -7,6 +7,11 @@
 //     static native long schemaCreate(String[] names, int[] elemTypes, int[] depths, boolean[] nullable, int recordType);
 //     static native long schemaCreateFormat(String[] names, int[] elemTypes, int[] depths, boolean[] nullable, int recordType,
 //                                           String nestedArrayFormat);   // "featureList" (schemaCreate) or "ragged": TFR_S_RAGGED
+//     static native long schemaCreateOptions(String[] names, int[] elemTypes, int[] depths, boolean[] nullable, int recordType,
+//                                            String nestedArrayFormat, String extendedTypes);   // + extendedTypes "true": TFR_S_INT64_TYPES
+//     static native int extendedElemType(String typeName, String extendedTypes);   // DataType.typeName of boolean, byte, short,
+//                                                 // date, timestamp -> TFR_T_BOOL .. TFR_T_TIMESTAMP under "true"; -1 under "false"
+//                                                 // (unsupported, as in the reference); -2 another type; -3 another option value
 //     static native int udtElemType(String udtClassName);   // a UserDefinedType's TFR_T_* by class name (VectorUDT: 10), -1 none
 //     static native int udtElemTypeFormat(String udtClassName, String vectorFormat);   // the same under the vectorFormat option:
 //                                                 // VectorUDT 10 (dense) or 11 (sparse), -1 another UDT, -2 another format
@@ -123,6 +128,48 @@ extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_
     return 0;
   }
   return schema_create(env, names, elemTypes, depths, nullable, recordType, (uint32_t)flags);
+}
+// DefaultSource's extendedTypes option (include/tfrgpu.h, INT64 TYPES) as schema flags: "false" (the default) 0, "true"
+// TFR_S_INT64_TYPES; -1 (IllegalArgumentException) for any other value
+static int64_t extended_types_flags(const std::string& value) {
+  if (value == "false") return 0;
+  if (value == "true") return TFR_S_INT64_TYPES;
+  return -1;
+}
+// The element type of a Spark field by its DataType.typeName under the extendedTypes option: boolean, byte, short, date and
+// timestamp are TFR_T_BOOL .. TFR_T_TIMESTAMP with "true", -1 (unsupported, as in the reference) with "false"; -2 for any other
+// type name (the glue's own mapping applies); -3 for an option value other than these, which the glue refuses before any work
+static int32_t extended_elem_type(const std::string& type_name, const std::string& value) {
+  const int64_t flags = extended_types_flags(value);
+  if (flags < 0) return -3;
+  static const struct { const char* name; int32_t t; } M[] = {
+      {"boolean", TFR_T_BOOL}, {"byte", TFR_T_INT8}, {"short", TFR_T_INT16}, {"date", TFR_T_DATE}, {"timestamp", TFR_T_TIMESTAMP}};
+  for (const auto& m : M)
+    if (type_name == m.name) return flags ? m.t : -1;
+  return -2;
+}
+static std::string jstring_or(JNIEnv* env, jstring js, const char* dflt) {
+  const char* u = js ? env->GetStringUTFChars(js, nullptr) : nullptr;
+  const std::string out = u ? u : dflt;
+  if (u) env->ReleaseStringUTFChars(js, u);
+  return out;
+}
+extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_schemaCreateOptions(
+    JNIEnv* env, jclass, jobjectArray names, jintArray elemTypes, jintArray depths, jbooleanArray nullable, jint recordType,
+    jstring nestedArrayFormat, jstring extendedTypes) {
+  const std::string fmt = jstring_or(env, nestedArrayFormat, "featureList"), ext = jstring_or(env, extendedTypes, "false");
+  const int64_t nested = nested_array_flags(fmt, recordType), wide = extended_types_flags(ext);
+  if (nested < 0 || wide < 0) {
+    env->ThrowNew(env->FindClass("java/lang/IllegalArgumentException"),
+                  (nested < 0 ? "nestedArrayFormat " + fmt + ": featureList, or ragged for Example records"
+                              : "extendedTypes " + ext + ": the option takes true or false").c_str());
+    return 0;
+  }
+  return schema_create(env, names, elemTypes, depths, nullable, recordType, (uint32_t)(nested | wide));
+}
+extern "C" JNIEXPORT jint JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_extendedElemType(JNIEnv* env, jclass, jstring typeName,
+                                                                                                      jstring extendedTypes) {
+  return extended_elem_type(jstring_or(env, typeName, ""), jstring_or(env, extendedTypes, "false"));
 }
 // The element type of a UserDefinedType field, by the UDT's class name, so that the glue needs no compile-time dependency on
 // spark-mllib: both VectorUDTs (same sqlType) are TFR_T_VECTOR; any other UDT is -1 (unsupported, as in the reference).

@@ -7,6 +7,7 @@ lower to the C ABI's ``tfr_field`` (include/tfrgpu.h).  M/ = src/main/scala/com/
 """
 from __future__ import annotations
 
+import datetime as _dt
 from dataclasses import dataclass
 from typing import List, Sequence
 
@@ -20,6 +21,10 @@ TFR_T_SPARSE_VECTOR = 11                               # the same, as TF sparse 
 # the feature keys of a sparse vector `v`: v + suffix (TFR_SPARSE_*_SUFFIX of include/tfrgpu.h)
 SPARSE_INDICES_SUFFIX, SPARSE_VALUES_SUFFIX, SPARSE_SIZE_SUFFIX = "_indices", "_values", "_size"
 VECTOR_FORMATS = ("dense", "sparse")                   # the `vectorFormat` DataSource option; dense is the default
+# BooleanType, ByteType, ShortType, DateType, TimestampType: stored as Int64 features with the option extendedTypes=true
+# (include/tfrgpu.h, INT64 TYPES); refused without it
+TFR_T_BOOL, TFR_T_INT8, TFR_T_INT16, TFR_T_DATE, TFR_T_TIMESTAMP = 12, 13, 14, 15, 16
+INT64_TYPES = (TFR_T_BOOL, TFR_T_INT8, TFR_T_INT16, TFR_T_DATE, TFR_T_TIMESTAMP)
 TFR_T_UNSUPPORTED = 99
 TFR_RT_EXAMPLE, TFR_RT_SEQUENCE_EXAMPLE, TFR_RT_BYTE_ARRAY = range(3)
 
@@ -162,11 +167,72 @@ def _to_sparse(size: int, indices: np.ndarray, values: np.ndarray) -> SparseVect
 
 
 class TimestampType(DataType):
-    """Exists only so the reference's "unsupported data type" tests can be restated."""
+    """Microseconds since the epoch, UTC; a Python value is a datetime with tzinfo=timezone.utc.  Only with extendedTypes=true
+    (include/tfrgpu.h, INT64 TYPES); the reference refuses it."""
+    int64_id = TFR_T_TIMESTAMP
 
 
 class BooleanType(DataType):
-    pass
+    """Only with extendedTypes=true (include/tfrgpu.h, INT64 TYPES); the reference refuses it."""
+    int64_id = TFR_T_BOOL
+
+
+class ByteType(DataType):
+    """Only with extendedTypes=true (include/tfrgpu.h, INT64 TYPES)."""
+    int64_id = TFR_T_INT8
+
+
+class ShortType(DataType):
+    """Only with extendedTypes=true (include/tfrgpu.h, INT64 TYPES)."""
+    int64_id = TFR_T_INT16
+
+
+class DateType(DataType):
+    """Days since 1970-01-01; a Python value is a datetime.date.  Only with extendedTypes=true (include/tfrgpu.h, INT64 TYPES)."""
+    int64_id = TFR_T_DATE
+
+
+_EPOCH_DATE = _dt.date(1970, 1, 1)
+_EPOCH = _dt.datetime(1970, 1, 1, tzinfo=_dt.timezone.utc)
+_RANGE = {TFR_T_INT8: (-128, 127), TFR_T_INT16: (-32768, 32767)}
+
+
+def int64_leaf(t: int, v) -> int:
+    """A Python value of INT64 TYPES type t -> the leaf value its column holds (bool: 0 / 1, byte / short: the int, date: days,
+    timestamp: microseconds, UTC).  A byte or short out of range, a naive datetime, or a value of the wrong kind is ValueError."""
+    if t == TFR_T_BOOL:
+        if not isinstance(v, (bool, int, np.bool_, np.integer)):
+            raise ValueError(f"BooleanType takes bool, not {type(v).__name__}")
+        return 1 if v else 0
+    if t in _RANGE:
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+            raise ValueError(f"{'ByteType' if t == TFR_T_INT8 else 'ShortType'} takes int, not {type(v).__name__}")
+        lo, hi = _RANGE[t]
+        if not lo <= int(v) <= hi:
+            raise ValueError(f"{int(v)} is outside [{lo}, {hi}]")
+        return int(v)
+    if t == TFR_T_DATE:
+        if isinstance(v, _dt.datetime) or not isinstance(v, _dt.date):
+            raise ValueError(f"DateType takes datetime.date, not {type(v).__name__}")
+        return (v - _EPOCH_DATE).days
+    if t == TFR_T_TIMESTAMP:
+        if not isinstance(v, _dt.datetime):
+            raise ValueError(f"TimestampType takes datetime.datetime, not {type(v).__name__}")
+        if v.tzinfo is None or v.utcoffset() is None:
+            raise ValueError("TimestampType takes a timezone-aware datetime (tzinfo=timezone.utc); a naive one is ambiguous")
+        return (v - _EPOCH) // _dt.timedelta(microseconds=1)
+    raise ValueError(f"type id {t} is not one of INT64_TYPES")
+
+
+def int64_value(t: int, x: int):
+    """The leaf value x of an INT64 TYPES column of type t -> its Python value (int64_leaf's inverse)."""
+    if t == TFR_T_BOOL:
+        return bool(x)
+    if t == TFR_T_DATE:
+        return _EPOCH_DATE + _dt.timedelta(days=int(x))
+    if t == TFR_T_TIMESTAMP:
+        return _EPOCH + _dt.timedelta(microseconds=int(x))
+    return int(x)
 
 
 class ArrayType(DataType):
@@ -223,10 +289,11 @@ def check_vector_format(vector_format: str) -> str:
     return vector_format
 
 
-def lower_type(dt: DataType, vector_format: str = "dense"):
+def lower_type(dt: DataType, vector_format: str = "dense", extended_types: bool = False):
     """DataType -> (elem_type_id, depth).  Anything the reference rejects lowers to
     (TFR_T_UNSUPPORTED, depth) and is refused by tfr_schema_create; so is ArrayType(VectorUDT), (TFR_T_VECTOR, depth > 0).
-    A VectorUDT is TFR_T_VECTOR, or TFR_T_SPARSE_VECTOR with vector_format="sparse"."""
+    A VectorUDT is TFR_T_VECTOR, or TFR_T_SPARSE_VECTOR with vector_format="sparse".  BooleanType, ByteType, ShortType,
+    DateType and TimestampType are their INT64_TYPES id with extended_types (the option extendedTypes=true), else unsupported."""
     check_vector_format(vector_format)
     depth = 0
     while isinstance(dt, ArrayType):
@@ -234,6 +301,8 @@ def lower_type(dt: DataType, vector_format: str = "dense"):
         dt = dt.elementType
     if dt.tfr_id == TFR_T_VECTOR and vector_format == "sparse":
         return TFR_T_SPARSE_VECTOR, depth
+    if extended_types and getattr(dt, "int64_id", None):
+        return dt.int64_id, depth
     return dt.tfr_id, depth
 
 
