@@ -180,10 +180,25 @@ enum {
  *              lists) is TFR_E_INVALID_ARG at the first such row.
  *   - Paths  : every decode path takes ragged fields (tile, large-record, general, pipelined submit).  The tile and large-record
  *              kernels do not check the parts; a batch whose parts disagree goes to the general path, which reports it.
- * These rules restate TensorFlow's tf.io.RaggedFeature documentation and are NOT checked against TensorFlow or a JVM.          */
+ *   - Row splits : the DataSource option raggedPartition=rowSplits (`rowLengths`, the default, is the layout above; any other
+ *              value, or rowSplits without nestedArrayFormat=ragged, is IllegalArgumentException before any work) is
+ *              TFR_S_RAGGED | TFR_S_RAGGED_ROW_SPLITS (TFR_S_RAGGED_ROW_SPLITS alone is TFR_E_INVALID_ARG).  The partition is
+ *              RaggedFeature.RowSplits(x_row_splits), the encoding tf.RaggedTensor holds (rt.row_splits):
+ *     <name>TFR_RAGGED_ROW_SPLITS_SUFFIX   Int64List           k + 1 entries 0, l0, l0+l1, .., the sum, for k inner lists
+ *              in place of the lengths part, with its place in the lowering, its nullability and its key-collision rule.
+ *              Write: null x omits both features; [] writes an empty values list and the splits [0]; [[]] the splits [0, 0].
+ *              Read, both parts present: the splits must have at least one entry (an empty list is an error here, unlike the
+ *              lengths), a first entry 0, no decreasing entry and a last entry equal to the number of values, else
+ *              TFR_E_BAD_NESTING at x.  Absence, precedence and every other rule are the lengths part's.  So a file written with
+ *              the other partition reads as TFR_E_BAD_NESTING (x_values present, the expected partition absent): lengths are
+ *              never read as splits, nor splits as lengths.
+ * These rules restate TensorFlow's tf.io.RaggedFeature and RaggedTensor.from_row_splits documentation and are NOT checked against
+ * TensorFlow or a JVM.                                                                                                         */
 #define TFR_RAGGED_VALUES_SUFFIX      "_values"
 #define TFR_RAGGED_ROW_LENGTHS_SUFFIX "_row_lengths"
+#define TFR_RAGGED_ROW_SPLITS_SUFFIX  "_row_splits"
 #define TFR_S_RAGGED 0x1u
+#define TFR_S_RAGGED_ROW_SPLITS 0x8u
 
 /* INT64 TYPES: the DataSource option extendedTypes=true (`false`, the default, refuses these types as before; any other value is
  * IllegalArgumentException before any work) is tfr_schema_create_ex with TFR_S_INT64_TYPES, which may be combined with
@@ -248,7 +263,7 @@ const char* tfr_last_error(void);
  * `fields` are ignored.                                                                                              */
 int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, int32_t record_type,
                           tfr_schema** out);
-/* tfr_schema_create with schema flags: TFR_S_RAGGED (RAGGED above), TFR_S_INT64_TYPES (INT64 TYPES above); any other bit is TFR_E_INVALID_ARG.  tfr_schema_create is
+/* tfr_schema_create with schema flags: TFR_S_RAGGED and TFR_S_RAGGED_ROW_SPLITS (RAGGED above), TFR_S_INT64_TYPES (INT64 TYPES above); any other bit is TFR_E_INVALID_ARG.  tfr_schema_create is
  * this call with flags 0.                                                                                              */
 int32_t tfr_schema_create_ex(const tfr_field* fields, int32_t n_fields, int32_t record_type, uint32_t schema_flags,
                              tfr_schema** out);

@@ -75,6 +75,9 @@ _LEAF_DTYPE = {TFR_T_INT32: np.int32, TFR_T_INT64: np.int64, TFR_T_FLOAT32: np.f
 TFR_S_RAGGED = 0x1
 TFR_RAGGED_VALUES_SUFFIX = "_values"
 TFR_RAGGED_ROW_LENGTHS_SUFFIX = "_row_lengths"
+# ... and of raggedPartition=rowSplits, with TFR_S_RAGGED: the partition stored as row splits
+TFR_S_RAGGED_ROW_SPLITS = 0x8
+TFR_RAGGED_ROW_SPLITS_SUFFIX = "_row_splits"
 # INT64 TYPES (include/tfrgpu.h): the schema flag of extendedTypes=true
 TFR_S_INT64_TYPES = 0x4
 

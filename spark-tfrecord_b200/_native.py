@@ -11,7 +11,7 @@ from typing import List, Optional
 import numpy as np
 
 from . import _cabi as A
-from ._cabi import TFR_S_INT64_TYPES, TFR_S_RAGGED, HostColumn, column_from_ctypes, make_fields, tfr_batch_info, tfr_column, tfr_field
+from ._cabi import TFR_S_INT64_TYPES, TFR_S_RAGGED, TFR_S_RAGGED_ROW_SPLITS, HostColumn, column_from_ctypes, make_fields, tfr_batch_info, tfr_column, tfr_field
 from .sqltypes import StructType
 
 _DIR = os.path.dirname(os.path.abspath(__file__))
@@ -181,18 +181,19 @@ def _check(rc: int):
 
 class Schema:
     def __init__(self, schema: StructType, record_type: int = 0, vector_format: str = "dense", ragged: bool = False,
-                 extended_types: bool = False):
+                 extended_types: bool = False, row_splits: bool = False):
         """`vector_format`: the `vectorFormat` option, how VectorUDT fields are stored (include/tfrgpu.h, VECTORS and SPARSE
         VECTORS); "sparse" lowers each to three fields (sqltypes.lowered_schema), and the columns follow the lowered schema.
         `ragged`: the option nestedArrayFormat=ragged (TFR_S_RAGGED, include/tfrgpu.h RAGGED); a nested array stays one
         column.  `extended_types`: the option extendedTypes=true (TFR_S_INT64_TYPES, include/tfrgpu.h INT64 TYPES): BooleanType,
-        ByteType, ShortType, DateType and TimestampType are stored as Int64 features."""
+        ByteType, ShortType, DateType and TimestampType are stored as Int64 features.  `row_splits`: the option
+        raggedPartition=rowSplits (TFR_S_RAGGED_ROW_SPLITS, with `ragged`): the partition is x_row_splits, not x_row_lengths."""
         self.struct = schema
         self.record_type = record_type
         self.vector_format = vector_format
         fields, self._keep = make_fields(schema, vector_format, extended_types)
         h = C.c_void_p()
-        flags = (TFR_S_RAGGED if ragged else 0) | (TFR_S_INT64_TYPES if extended_types else 0)
+        flags = (TFR_S_RAGGED if ragged else 0) | (TFR_S_INT64_TYPES if extended_types else 0) | (TFR_S_RAGGED_ROW_SPLITS if row_splits else 0)
         _check(lib().tfr_schema_create_ex(fields, len(schema), record_type, flags, C.byref(h)))
         self.h = h
 
@@ -364,10 +365,10 @@ class Batch:
 class Decoder:
     def __init__(self, schema: StructType, record_type: int = 0, device: int = 0, flags: int = A.TFR_F_DEFAULT,
                  corrupt_field: Optional[int] = None, vector_format: str = "dense", ragged: bool = False,
-                 extended_types: bool = False):
+                 extended_types: bool = False, row_splits: bool = False):
         """`corrupt_field`: with TFR_F_PERMISSIVE in `flags`, the index of the schema field that receives a failing record's
         payload (a nullable BinaryType column; tfr_decoder_create_permissive).  `vector_format`: as Schema's."""
-        self.schema = Schema(schema, record_type, vector_format, ragged, extended_types)
+        self.schema = Schema(schema, record_type, vector_format, ragged, extended_types, row_splits)
         self.ncols = lib().tfr_schema_num_fields(self.schema.h)     # ByteArray: byteArray, then the generated fields
         h = C.c_void_p()
         if corrupt_field is None:
@@ -453,8 +454,8 @@ class Decoder:
 
 class Encoder:
     def __init__(self, schema: StructType, record_type: int = 0, device: int = 0, flags: int = 0, vector_format: str = "dense",
-                 ragged: bool = False, extended_types: bool = False):
-        self.schema = Schema(schema, record_type, vector_format, ragged, extended_types)
+                 ragged: bool = False, extended_types: bool = False, row_splits: bool = False):
+        self.schema = Schema(schema, record_type, vector_format, ragged, extended_types, row_splits)
         self.ncols = 1 if record_type == 2 else lib().tfr_schema_num_fields(self.schema.h)   # (a sparse vector adds two)
         h = C.c_void_p()
         _check(lib().tfr_encoder_create(self.schema.h, device, flags, C.byref(h)))

@@ -219,6 +219,7 @@ struct tfr_schema {
   std::vector<int32_t> rag_len;
   int32_t n_rag = 0;
   bool ragged(int32_t f) const { return f >= 0 && f < (int32_t)rag_len.size() && rag_len[f] >= 0; }
+  bool rag_splits = false;           // the parts rag_len[x] are row splits (TFR_S_RAGGED_ROW_SPLITS), not row lengths
   int32_t n_cols() const { return (int32_t)fields.size() - n_rag; }
   // the same fields without the ragged lowering (x at depth 2), which the UnsafeRow encoders take rows apart by
   std::shared_ptr<tfr_schema> plain;
@@ -263,7 +264,9 @@ extern "C" int32_t tfr_schema_create(const tfr_field* fields, int32_t n_fields, 
 extern "C" int32_t tfr_schema_create_ex(const tfr_field* fields, int32_t n_fields, int32_t record_type, uint32_t schema_flags,
                                         tfr_schema** out) {
   if (!out || n_fields < 0 || (n_fields > 0 && !fields)) return fail(TFR_E_INVALID_ARG, "null argument");
-  if (schema_flags & ~(TFR_S_RAGGED | TFR_S_INT64_TYPES)) return fail(TFR_E_INVALID_ARG, "unknown schema flags");
+  if (schema_flags & ~(TFR_S_RAGGED | TFR_S_INT64_TYPES | TFR_S_RAGGED_ROW_SPLITS)) return fail(TFR_E_INVALID_ARG, "unknown schema flags");
+  if ((schema_flags & TFR_S_RAGGED_ROW_SPLITS) && !(schema_flags & TFR_S_RAGGED))
+    return fail(TFR_E_INVALID_ARG, "raggedPartition=rowSplits needs nestedArrayFormat=ragged");
   if (record_type < TFR_RT_EXAMPLE || record_type > TFR_RT_BYTE_ARRAY)
     return fail(TFR_E_BAD_RECORD_TYPE, "Unsupported recordType: recordType can be ByteArray, Example or SequenceExample");
   if ((schema_flags & TFR_S_RAGGED) && record_type == TFR_RT_SEQUENCE_EXAMPLE)
@@ -360,9 +363,10 @@ extern "C" int32_t tfr_schema_create_ex(const tfr_field* fields, int32_t n_field
     add(user[v] + TFR_SPARSE_INDICES_SUFFIX, TFR_T_INT32, 1, true, VK_INDICES, v);
     add(user[v] + TFR_SPARSE_SIZE_SUFFIX, TFR_T_INT32, 0, true, VK_SIZE, v);
   }
+  s->rag_splits = (schema_flags & TFR_S_RAGGED_ROW_SPLITS) != 0;
   for (int32_t x : ragged) {
     s->rag_len[x] = (int32_t)s->fields.size();
-    add(user[x] + TFR_RAGGED_ROW_LENGTHS_SUFFIX, TFR_T_INT64, 1, true, VK_NONE, x);
+    add(user[x] + (s->rag_splits ? TFR_RAGGED_ROW_SPLITS_SUFFIX : TFR_RAGGED_ROW_LENGTHS_SUFFIX), TFR_T_INT64, 1, true, VK_NONE, x);
   }
   s->n_rag = (int32_t)ragged.size();
   if (s->n_rag) {

@@ -412,6 +412,56 @@ __device__ __forceinline__ uint64_t ragged_lengths_sum(const uint8_t* data, uint
   return bad ? ~0ull : sum;
 }
 
+// the row-splits partition's consistency check (TFR_S_RAGGED_ROW_SPLITS): true when the splits part's values in row `row` (the
+// final run of the winning entry, by Feature's merge rules, as in ragged_lengths_sum) are at least one entry, the first 0, none
+// decreasing and the last `n_values`.  `src`, `canon`, `count` as there.
+__device__ __forceinline__ bool ragged_splits_ok(const uint8_t* data, uint32_t nbytes, uint32_t src, bool canon, uint32_t count,
+                                                 uint32_t n_values) {
+  uint32_t m = 0;
+  int64_t first = 0, last = 0;
+  bool dec = false;
+  auto add = [&](uint64_t u) { const int64_t v = (int64_t)u; if (m == 0) first = v; else if (v < last) dec = true; last = v; ++m; };
+  if (canon) {
+    Cur pk{data + src, data + nbytes};
+    for (uint32_t i = 0; i < count; ++i) { uint64_t v; if (!rd_varint64(pk, v)) return false; add(v); }
+  } else {
+    Cur c{data + src, data + nbytes};
+    uint32_t l;
+    if (!rd_len(c, l)) return false;
+    Cur e{c.p, c.p + l};
+    for (;;) {                                                 // MapEntry: value = 2 (repeated occurrences merge)
+      uint32_t tag;
+      if (!rd_tag(e, tag)) return false;
+      if (tag == 0) break;
+      if (tag != 0x12) { if (!skip_field(e, tag)) return false; continue; }
+      if (!rd_len(e, l)) return false;
+      Cur f{e.p, e.p + l};
+      e.p += l;
+      for (;;) {                                               // Feature: bytes_list = 1, float_list = 2, int64_list = 3
+        if (!rd_tag(f, tag)) return false;
+        if (tag == 0) break;
+        if (tag != 0x0A && tag != 0x12 && tag != 0x1A) { if (!skip_field(f, tag)) return false; continue; }
+        if (!rd_len(f, l)) return false;
+        Cur b{f.p, f.p + l};
+        f.p += l;
+        if (tag != 0x1A) { m = 0; dec = false; continue; }    // the oneof switches: the int64 values before it are discarded
+        for (;;) {                                             // Int64List: value = 1, packed or not
+          if (!rd_tag(b, tag)) return false;
+          if (tag == 0) break;
+          if (tag == 0x08) { uint64_t v; if (!rd_varint64(b, v)) return false; add(v); }
+          else if (tag == 0x0A) {
+            if (!rd_len(b, l)) return false;
+            Cur pk{b.p, b.p + l};
+            while (pk.p < pk.end) { uint64_t v; if (!rd_varint64(pk, v)) return false; add(v); }
+            b.p += l;
+          } else if (!skip_field(b, tag)) return false;
+        }
+      }
+    }
+  }
+  return m > 0 && first == 0 && !dec && last == (int64_t)n_values;
+}
+
 // a row that fails before the per-field epilogue (bad CRC, malformed proto): zero counts, null validity
 __device__ __forceinline__ void null_fill_row(const DecodeArgs& A, uint32_t row) {
   const uint32_t lane = threadIdx.x & 31;
@@ -419,9 +469,10 @@ __device__ __forceinline__ void null_fill_row(const DecodeArgs& A, uint32_t row)
   for (uint32_t c = lane; c < (uint32_t)A.sch.n_cnt; c += 32) A.cnt[(size_t)c * A.n + row] = 0;
 }
 
-// RG: the schema has ragged fields, whose parts must agree (RAGGED, include/tfrgpu.h); without them the kernel is unchanged
-template <bool RG>
-__global__ void __launch_bounds__(256) decode_pass1_kernel(DecodeArgs A) {
+// RG: the schema has ragged fields, whose parts must agree (RAGGED, include/tfrgpu.h); without them the kernel is unchanged.
+// RS: they are stored with row splits (TFR_S_RAGGED_ROW_SPLITS), decode_pass1_splits_kernel.
+template <bool RG, bool RS>
+__device__ __forceinline__ void decode_pass1(const DecodeArgs& A) {
   extern __shared__ uint32_t smem[];
   uint32_t* stab = smem;
   crc_stage_tables(stab, A.tabs);
@@ -517,8 +568,13 @@ __global__ void __launch_bounds__(256) decode_pass1_kernel(DecodeArgs A) {
           if (px && pl) {
             const DevField& fl = A.sch.fields[L];
             const size_t vs = (size_t)fl.var_slot * A.n + row;
-            const uint64_t sum = ragged_lengths_sum(A.data, A.nbytes, A.src[vs], A.cflag[vs] == CF_CANON, A.cnt[(size_t)fl.cnt_slot * A.n + row]);
-            mis = sum != (uint64_t)A.cnt[(size_t)A.sch.fields[x].cnt_slot * A.n + row];
+            if constexpr (RS) {
+              mis = !ragged_splits_ok(A.data, A.nbytes, A.src[vs], A.cflag[vs] == CF_CANON, A.cnt[(size_t)fl.cnt_slot * A.n + row],
+                                      A.cnt[(size_t)A.sch.fields[x].cnt_slot * A.n + row]);
+            } else {
+              const uint64_t sum = ragged_lengths_sum(A.data, A.nbytes, A.src[vs], A.cflag[vs] == CF_CANON, A.cnt[(size_t)fl.cnt_slot * A.n + row]);
+              mis = sum != (uint64_t)A.cnt[(size_t)A.sch.fields[x].cnt_slot * A.n + row];
+            }
           }
           if (mis) bad = min(bad, (uint32_t)x);
         }
@@ -530,6 +586,9 @@ __global__ void __launch_bounds__(256) decode_pass1_kernel(DecodeArgs A) {
     if (lane == 0) A.status[row] = worst == 0xffffffffu ? 0u : ((worst & 0xff) | (((worst >> 8) + 1) << 8));
   }
 }
+template <bool RG>
+__global__ void __launch_bounds__(256) decode_pass1_kernel(DecodeArgs A) { decode_pass1<RG, false>(A); }
+__global__ void __launch_bounds__(256) decode_pass1_splits_kernel(DecodeArgs A) { decode_pass1<true, true>(A); }
 
 // ---------------------------------------------------------------------------------------------
 // pass 2: emit variable-width cells

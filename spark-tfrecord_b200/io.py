@@ -83,6 +83,18 @@ def _nested_array_format(options: Optional[Dict[str, str]]) -> bool:
     return nf == "ragged"
 
 
+def _ragged_partition(options: Optional[Dict[str, str]]) -> bool:
+    """the `raggedPartition` option: True for "rowSplits", where a ragged field's partition is x_row_splits (the k + 1 entries
+    0, l0, l0+l1, .. of RaggedFeature.RowSplits) instead of x_row_lengths; "rowLengths" (the default) is the layout of
+    _nested_array_format.  Anything else, and rowSplits without nestedArrayFormat=ragged, is refused before any work."""
+    value = (options or {}).get("raggedPartition", "rowLengths")
+    if value not in ("rowLengths", "rowSplits"):
+        raise _native.IllegalArgumentException(-1, f"raggedPartition {value}: the option takes rowLengths or rowSplits")
+    if value == "rowSplits" and not _nested_array_format(options):
+        raise _native.IllegalArgumentException(-1, "raggedPartition=rowSplits needs nestedArrayFormat=ragged")
+    return value == "rowSplits"
+
+
 def _extended_types(options: Optional[Dict[str, str]]) -> bool:
     """the `extendedTypes` option: "true" reads and writes BooleanType, ByteType, ShortType, DateType and TimestampType fields
     (and arrays of them) as Int64 features (include/tfrgpu.h, INT64 TYPES); "false" (the default) refuses them, as the
@@ -494,6 +506,7 @@ class TFRecordFileReader:
         rt = _record_type(options)
         vf = _vector_format(options)
         ragged = _nested_array_format(options)
+        splits = _ragged_partition(options)
         ext = _extended_types(options)
         flags, corrupt = _read_mode(options, schema if dataSchema is None else dataSchema, schema)
         block = block_bytes or TFRecordFileReader.BLOCK_BYTES
@@ -501,7 +514,7 @@ class TFRecordFileReader:
         split = (_record_index(options) and _codec_of_path(file.toPath()) is None
                  and (file.start, file.length) != (0, os.path.getsize(file.toPath())))
         dec = _native.Decoder(_decoder_schema(schema), rt, device, flags, corrupt_field=corrupt, vector_format=vf, ragged=ragged,
-                              extended_types=ext)
+                              extended_types=ext, row_splits=splits)
 
         def gen():
             todo = []
@@ -610,7 +623,8 @@ class TFRecordOutputWriter:
         self.schema = byte_array_schema() if self.recordType == 2 else dataSchema
         self.vectorFormat = _vector_format(options)
         self._enc = _native.Encoder(self.schema, self.recordType, device, vector_format=self.vectorFormat,
-                                    ragged=_nested_array_format(options), extended_types=_extended_types(options))
+                                    ragged=_nested_array_format(options), extended_types=_extended_types(options),
+                                    row_splits=_ragged_partition(options))
         self._rows: List[tuple] = []
         self._bytes = 0
         codec = _codec_name((options or {}).get("codec", ""))
@@ -737,6 +751,7 @@ class DefaultSource:
         reads the files back under the options it was inferred with (buildReader refuses PERMISSIVE without it)."""
         from .sharding import allreduce_schema, codes_to_struct, shard_lpt
         _nested_array_format(options)                 # validated; a ragged file infers as its two plain fields
+        _ragged_partition(options)                    # (row splits alike)
         _extended_types(options)                      # validated; an Int64List still infers as LongType
         mode, flags = _mode_flags(options)
         rt = _record_type(options)
@@ -798,6 +813,7 @@ class DefaultSource:
         _read_mode(options, dataSchema, requiredSchema)
         _vector_format(options)
         _nested_array_format(options)
+        _ragged_partition(options)
         _extended_types(options)
         _record_index(options)
         return lambda file: TFRecordFileReader.readFile(None, options, file, requiredSchema, device, dataSchema=dataSchema)
@@ -806,6 +822,7 @@ class DefaultSource:
         codec = _codec_name((options or {}).get("codec", ""))             # :94-102: the option turns output compression on
         _vector_format(options)
         _nested_array_format(options)
+        _ragged_partition(options)
         _extended_types(options)
         _check_record_index(options, codec)
 

@@ -9,6 +9,9 @@
 //                                           String nestedArrayFormat);   // "featureList" (schemaCreate) or "ragged": TFR_S_RAGGED
 //     static native long schemaCreateOptions(String[] names, int[] elemTypes, int[] depths, boolean[] nullable, int recordType,
 //                                            String nestedArrayFormat, String extendedTypes);   // + extendedTypes "true": TFR_S_INT64_TYPES
+//     static native long schemaCreatePartition(String[] names, int[] elemTypes, int[] depths, boolean[] nullable, int recordType,
+//                                              String nestedArrayFormat, String extendedTypes, String raggedPartition);
+//                                                 // + raggedPartition "rowSplits" (with "ragged"): TFR_S_RAGGED_ROW_SPLITS
 //     static native int extendedElemType(String typeName, String extendedTypes);   // DataType.typeName of boolean, byte, short,
 //                                                 // date, timestamp -> TFR_T_BOOL .. TFR_T_TIMESTAMP under "true"; -1 under "false"
 //                                                 // (unsupported, as in the reference); -2 another type; -3 another option value
@@ -166,6 +169,29 @@ extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_
     return 0;
   }
   return schema_create(env, names, elemTypes, depths, nullable, recordType, (uint32_t)(nested | wide));
+}
+// DefaultSource's raggedPartition option (include/tfrgpu.h, RAGGED, Row splits) as schema flags, given nestedArrayFormat's
+// (`nested`, nested_array_flags): "rowLengths" (the default) 0, "rowSplits" TFR_S_RAGGED_ROW_SPLITS when nested has TFR_S_RAGGED;
+// -1 (IllegalArgumentException) for any other value, and for rowSplits without ragged
+static int64_t ragged_partition_flags(const std::string& value, int64_t nested) {
+  if (value == "rowLengths") return 0;
+  if (value == "rowSplits" && nested >= 0 && (nested & TFR_S_RAGGED)) return TFR_S_RAGGED_ROW_SPLITS;
+  return -1;
+}
+extern "C" JNIEXPORT jlong JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_schemaCreatePartition(
+    JNIEnv* env, jclass, jobjectArray names, jintArray elemTypes, jintArray depths, jbooleanArray nullable, jint recordType,
+    jstring nestedArrayFormat, jstring extendedTypes, jstring raggedPartition) {
+  const std::string fmt = jstring_or(env, nestedArrayFormat, "featureList"), ext = jstring_or(env, extendedTypes, "false"),
+                    part = jstring_or(env, raggedPartition, "rowLengths");
+  const int64_t nested = nested_array_flags(fmt, recordType), wide = extended_types_flags(ext), split = ragged_partition_flags(part, nested);
+  if (nested < 0 || wide < 0 || split < 0) {
+    env->ThrowNew(env->FindClass("java/lang/IllegalArgumentException"),
+                  (nested < 0 ? "nestedArrayFormat " + fmt + ": featureList, or ragged for Example records"
+                   : wide < 0 ? "extendedTypes " + ext + ": the option takes true or false"
+                              : "raggedPartition " + part + ": rowLengths, or rowSplits with nestedArrayFormat=ragged").c_str());
+    return 0;
+  }
+  return schema_create(env, names, elemTypes, depths, nullable, recordType, (uint32_t)(nested | wide | split));
 }
 extern "C" JNIEXPORT jint JNICALL Java_com_linkedin_spark_datasources_tfrecord_TfrGpu_extendedElemType(JNIEnv* env, jclass, jstring typeName,
                                                                                                       jstring extendedTypes) {

@@ -9,7 +9,11 @@ Then, the arms alternated rep by rep after a warm-up (medians, CUDA events aroun
   - resident decode GB/s (device input) with the ragged schema, and with the two plain fields per ragged field;
   - the assembly kernel's time (torch.profiler, a run of its own);
   - encode GB/s of framed output for host columns (tfr_encode) and for host UnsafeRows (tfr_encode_rows).
-Prints one JSON line with the card's name and power limit, read in the same call."""
+Prints one JSON line with the card's name and power limit, read in the same call.
+
+--partition rowSplits (raggedPartition=rowSplits) checks the same outputs for the row-splits layout too (bytes against
+tests/ragged_splits_rows.py, the ragged decode, the plain decode's splits part, tfr_encode_rows), then alternates the lengths
+and the splits layout on the same records: resident decode, the assembly kernels' time (ragged_*), and tfr_encode of columns."""
 import argparse
 import json
 import os
@@ -24,6 +28,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--records", type=int, default=1 << 20)
     ap.add_argument("--reps", type=int, default=7)
+    ap.add_argument("--partition", choices=["rowLengths", "rowSplits"], default="rowLengths")
     a = ap.parse_args()
     sys.path.insert(0, os.path.join(HERE, ".."))
     sys.path.insert(0, os.path.join(HERE, "..", "tests"))
@@ -81,6 +86,9 @@ def main():
     enc.encode_rows(rows, offs)
     assert enc.result_host() == data, "UnsafeRows encode differs from the columns encode"
 
+    if a.partition == "rowSplits":
+        return splits_arm(a, sch, cols, data, dev, dec_r, enc)
+
     # ---- times ----
     def timed(f):
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -117,6 +125,94 @@ def main():
                       "assembly_ms": asm, "decode_ragged_ms": med["decode_ragged"] * 1e3,
                       "encode_columns_GBps": len(data) / med["encode_columns"] / 1e9,
                       "encode_rows_GBps": len(data) / med["encode_rows"] / 1e9}))
+
+
+def _timed(torch, f):
+    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    s.record()
+    f()
+    e.record()
+    e.synchronize()
+    return s.elapsed_time(e) / 1e3
+
+
+def splits_arm(a, sch, cols, data_len, dev_len, dec_len, enc_len):
+    """--partition rowSplits: the row-splits layout checked, then timed against the lengths layout on the same records"""
+    import numpy as np
+    import torch
+    import ragged_splits_rows as RS
+    from spark_tfrecord_b200 import _cabi as A
+    from spark_tfrecord_b200 import _native
+    n = a.records
+    enc = _native.Encoder(sch, 0, ragged=True, row_splits=True)
+    data = enc.encode(cols)
+    m = min(n, 2000)
+    first = [tuple(c.get(r) for c in cols) for r in range(m)]
+    first = [(r[0], r[1], [[float(np.float32(v)) for v in i] for i in r[2]], r[3], r[4]) for r in first]
+    ref = RS.encode(sch, first)
+    assert data[:len(ref)] == ref, "row-splits bytes differ from the restatement"
+    dev = torch.from_numpy(np.frombuffer(data, dtype=np.uint8).copy()).cuda()
+    dec = _native.Decoder(sch, 0, ragged=True, row_splits=True)
+    b, _ = dec.decode(dev)
+    got = b.to_host()
+    assert b.info["error_code"] == 0 and b.n_rows == n
+    for c, g in zip(cols, got):
+        assert all(np.array_equal(o, go) for o, go in zip(c.offsets, g.offsets)) and np.array_equal(c.values, g.values)
+    rows, offs = b.unsafe_rows()
+    rows, offs = rows.copy(), offs.astype(np.int32)
+    b.release()
+    dec_p = _native.Decoder(RS.lowered_schema(sch), 0)
+    b, _ = dec_p.decode(dev)
+    got = b.to_host()
+    for j, c in ((1, cols[1]), (2, cols[2])):
+        sp = got[4 + j]
+        assert np.array_equal(sp.offsets[0], c.offsets[0] + np.arange(n + 1)), "one more entry per row"
+        o0, o1 = c.offsets[0].astype(np.int64), c.offsets[1].astype(np.int64)
+        k = np.diff(o0) + 1                                            # entries per row
+        row = np.repeat(np.arange(n), k)
+        at = np.arange(int(k.sum())) - np.repeat(np.cumsum(k) - k, k) + o0[row]
+        want = o1[at] - o1[o0[row]]
+        assert np.array_equal(sp.values, want)
+    b.release()
+    dec_p.close()
+    enc.encode_rows(rows, offs)
+    assert enc.result_host() == data, "UnsafeRows encode differs from the columns encode"
+    # the other partition's file: every record fails at x
+    b, _ = dec.decode(dev_len)
+    assert (b.info["error_code"], b.info["error_row"], b.info["error_field"]) == (A.TFR_E_BAD_NESTING, 0, 1)
+    b.release()
+
+    def dec_once(d, x):
+        bb, _ = d.decode(x)
+        bb.wait()
+        bb.release()
+
+    arms = {"decode_lengths": lambda: dec_once(dec_len, dev_len), "decode_splits": lambda: dec_once(dec, dev),
+            "encode_lengths": lambda: enc_len.encode(cols), "encode_splits": lambda: enc.encode(cols)}
+    for f in arms.values():
+        f(); f()
+    t = {k: [] for k in arms}
+    for _ in range(a.reps):
+        for k, f in arms.items():
+            t[k].append(_timed(torch, f))
+    from torch.profiler import ProfilerActivity, profile
+    asm = {}
+    for k, d, x in (("lengths", dec_len, dev_len), ("splits", dec, dev)):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            dec_once(d, x)
+        asm[k] = sum(ev.device_time_total for ev in prof.key_averages() if ev.key.startswith("ragged_")) / 1e3
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                         text=True).stdout.strip()
+    med = {k: statistics.median(v) for k, v in t.items()}
+    print(json.dumps({"gpu": gpu, "records": n, "framed_bytes_lengths": len(data_len), "framed_bytes_splits": len(data),
+                      "checked": True,
+                      "decode_lengths_GBps": len(data_len) / med["decode_lengths"] / 1e9,
+                      "decode_splits_GBps": len(data) / med["decode_splits"] / 1e9,
+                      "decode_lengths_ms": med["decode_lengths"] * 1e3, "decode_splits_ms": med["decode_splits"] * 1e3,
+                      "assembly_lengths_ms": asm["lengths"], "assembly_splits_ms": asm["splits"],
+                      "encode_lengths_GBps": len(data_len) / med["encode_lengths"] / 1e9,
+                      "encode_splits_GBps": len(data) / med["encode_splits"] / 1e9}))
 
 
 if __name__ == "__main__":
