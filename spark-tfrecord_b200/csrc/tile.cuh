@@ -265,6 +265,18 @@ __device__ __forceinline__ uint32_t crc_chunks(const uint32_t* g, const Tile& t,
   }
   return c;
 }
+// x^(8*16*m) mod P for m >= 512, past the xp16 table: a packed tile can hold one record of 8 KiB and more, whose leading CRC
+// warps shift further.  x^(8*16*m) = xp16[511]^q * xp16[m - 511 q]: one more GF(2) multiply per 511 chunks (8 KiB).  Out of
+// line, so that the common case (an xp16 lookup) keeps the CRC warps' code and registers as they are.
+__device__ __noinline__ uint32_t chunk_shift_far(const uint32_t* xp16, uint32_t m) {
+  uint32_t f = xp16[511];
+  for (m -= 511u; m; ) {
+    const uint32_t s = min(m, 511u);
+    f = gf2_mulmod(f, xp16[s]);
+    m -= s;
+  }
+  return f;
+}
 
 // shared memory layout (dynamic), all sections 16-byte aligned:
 //   [0,16) mbarrier | CRC tables g5 2 KiB + xp16 2 KiB | seen words [32][4] u32 + CRC accumulators [32] | DevField[nf] | FieldTemplate[nf] | names | entry table | tile bytes
@@ -445,7 +457,7 @@ __global__ void __launch_bounds__((PW + CW) * 32, (PW >= 16 ? 2 : PW >= 12 ? TIL
       }
       const uint32_t k0 = K * cw / CW, k1 = K * (cw + 1) / CW;
       c = crc_chunks(s8, T, b0 + 16 * k0, k1 - k0, c);
-      if (c) atomicXor(&scrc[lane], K - k1 ? gf2_mulmod(xp16[K - k1], c) : c);
+      if (c) atomicXor(&scrc[lane], K - k1 ? gf2_mulmod(K - k1 < 512u ? xp16[K - k1] : chunk_shift_far(xp16, K - k1), c) : c);
     }
     asm volatile("bar.sync 2, %0;" ::"r"(CW * 32) : "memory");
     if (cw == 0 && on) {
