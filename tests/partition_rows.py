@@ -95,18 +95,24 @@ def _write_partition(w: _Writer, k: int, t, v):
         w.slot(k, int.from_bytes(b + bytes(8 - len(b)), "little"))
 
 
-def joined_row(data_schema: StructType, data_row: Sequence, ptypes: Sequence, pvalues: Sequence) -> bytes:
+def write_data_field(w: _Writer, i: int, f, v):
+    """data field i of value v, as oracle.unsaferow.unsafe_row writes it"""
+    t, depth = lower_type(f.dataType)
+    if v is None or t == TFR_T_NULL:
+        w.set_null(i)
+    elif depth == 0 and t not in (TFR_T_STRING, TFR_T_BINARY):
+        w.slot(i, U._scalar_bits(t, v))
+    else:
+        w.var(i, U._leaf_bytes(t, v) if depth == 0 else U.unsafe_array(t, depth, v))
+
+
+def joined_row(data_schema: StructType, data_row: Sequence, ptypes: Sequence, pvalues: Sequence,
+               write_field=write_data_field) -> bytes:
+    """`write_field(w, i, field, value)` writes one data field (tests/composed_rows.py passes the one of its lowerings)"""
     nd = len(data_schema)
     w = _Writer(nd + len(ptypes))
-    for i, f in enumerate(data_schema):                      # as oracle.unsaferow.unsafe_row
-        t, depth = lower_type(f.dataType)
-        v = data_row[i]
-        if v is None or t == TFR_T_NULL:
-            w.set_null(i)
-        elif depth == 0 and t not in (TFR_T_STRING, TFR_T_BINARY):
-            w.slot(i, U._scalar_bits(t, v))
-        else:
-            w.var(i, U._leaf_bytes(t, v) if depth == 0 else U.unsafe_array(t, depth, v))
+    for i, f in enumerate(data_schema):
+        write_field(w, i, f, data_row[i])
     for j, (t, v) in enumerate(zip(ptypes, pvalues)):
         _write_partition(w, nd + j, t, v)
     return w.row()
@@ -117,9 +123,10 @@ def partition_row(ptypes: Sequence, pvalues: Sequence) -> bytes:
     return joined_row(StructType([]), [], ptypes, pvalues)
 
 
-def joined_rows(data_schema: StructType, rows: Sequence[Sequence], ptypes, pvalues) -> Tuple[np.ndarray, np.ndarray]:
+def joined_rows(data_schema: StructType, rows: Sequence[Sequence], ptypes, pvalues,
+                write_field=write_data_field) -> Tuple[np.ndarray, np.ndarray]:
     """-> (row bytes as uint8, int64 offsets[n + 1]), rows back to back"""
-    parts: List[bytes] = [joined_row(data_schema, r, ptypes, pvalues) for r in rows]
+    parts: List[bytes] = [joined_row(data_schema, r, ptypes, pvalues, write_field) for r in rows]
     offs = np.zeros(len(parts) + 1, dtype=np.int64)
     offs[1:] = np.cumsum([len(p) for p in parts])
     return np.frombuffer(b"".join(parts), dtype=np.uint8).copy(), offs

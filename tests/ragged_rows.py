@@ -61,12 +61,10 @@ def raise_row(schema: StructType, lowered: Sequence) -> Tuple[Optional[tuple], O
     return tuple(out), None
 
 
-def read(schema: StructType, payload: bytes) -> Tuple[Optional[tuple], Optional[Tuple[int, int]]]:
-    """(row, None) or (None, (TFR_E_* code, reported field)) for one Example payload read with nestedArrayFormat=ragged.  An
-    error of the lowered parse comes first (a lengths part's at its ragged field); the consistency check last."""
-    low = lowered_schema(schema)
-    n = len(schema.fields)
-    rg = ragged_fields(schema)
+def parse_lowered(low: StructType, payload: bytes, unkeyed=()) -> Tuple[Optional[list], Optional[Tuple[int, int]]]:
+    """one Example payload parsed by the plain rules of every field of `low` (oracle/pyref), field by field in order: (values,
+    None), or (None, (TFR_E_* code, lowered field)) at the first field that fails.  A field in `unkeyed` is no feature's (a
+    generated field, the corrupt-record column): it is read as None and never fails."""
     ex = pyref.Example()
     try:
         ex.ParseFromString(payload)
@@ -74,11 +72,25 @@ def read(schema: StructType, payload: bytes) -> Tuple[Optional[tuple], Optional[
         return None, (A.TFR_E_MALFORMED_PROTO, -1)
     row = []
     for f_i, f in enumerate(low.fields):
+        if f_i in unkeyed:
+            row.append(None)
+            continue
         try:
             row.append(pyref.deserialize_example(StructType([f]), ex)[0])
         except pyref.RefError as e:
             code = {"NullPointerException": A.TFR_E_NULL_IN_NONNULL, "NoSuchElementException": A.TFR_E_EMPTY_SCALAR}.get(
                 e.java_class, A.TFR_E_KIND_MISMATCH)
-            return None, (code, rg[f_i - n] if f_i >= n else f_i)
+            return None, (code, f_i)
+    return row, None
+
+
+def read(schema: StructType, payload: bytes) -> Tuple[Optional[tuple], Optional[Tuple[int, int]]]:
+    """(row, None) or (None, (TFR_E_* code, reported field)) for one Example payload read with nestedArrayFormat=ragged.  An
+    error of the lowered parse comes first (a lengths part's at its ragged field); the consistency check last."""
+    n = len(schema.fields)
+    rg = ragged_fields(schema)
+    row, err = parse_lowered(lowered_schema(schema), payload)
+    if err is not None:
+        return None, (err[0], rg[err[1] - n] if err[1] >= n else err[1])
     r, bad = raise_row(schema, row)
     return (r, None) if bad is None else (None, (A.TFR_E_BAD_NESTING, bad))

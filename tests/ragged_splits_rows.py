@@ -63,21 +63,10 @@ def raise_row(schema: StructType, lowered: Sequence) -> Tuple[Optional[tuple], O
 def read(schema: StructType, payload: bytes) -> Tuple[Optional[tuple], Optional[Tuple[int, int]]]:
     """(row, None) or (None, (TFR_E_* code, reported field)) for one Example payload read with raggedPartition=rowSplits.  An
     error of the lowered parse comes first (a splits part's at its ragged field); the consistency check last."""
-    low = lowered_schema(schema)
     n = len(schema.fields)
     rg = ragged_fields(schema)
-    ex = pyref.Example()
-    try:
-        ex.ParseFromString(payload)
-    except Exception:
-        return None, (A.TFR_E_MALFORMED_PROTO, -1)
-    row = []
-    for f_i, f in enumerate(low.fields):
-        try:
-            row.append(pyref.deserialize_example(StructType([f]), ex)[0])
-        except pyref.RefError as e:
-            code = {"NullPointerException": A.TFR_E_NULL_IN_NONNULL, "NoSuchElementException": A.TFR_E_EMPTY_SCALAR}.get(
-                e.java_class, A.TFR_E_KIND_MISMATCH)
-            return None, (code, rg[f_i - n] if f_i >= n else f_i)
+    row, err = RR.parse_lowered(lowered_schema(schema), payload)
+    if err is not None:
+        return None, (err[0], rg[err[1] - n] if err[1] >= n else err[1])
     r, bad = raise_row(schema, row)
     return (r, None) if bad is None else (None, (A.TFR_E_BAD_NESTING, bad))
